@@ -191,6 +191,15 @@ __device__ __forceinline__ bool eig9_factor_reg(const double* A, int r, int lane
   return neg;
 }
 
+// The residual test accepts ANY eigenpair: a start vector without a component along v_min (L^-T e_8 misses v_min when
+// its last entry vanishes) converges to the next eigenvector.  x with Rayleigh quotient rho belongs to the smallest
+// eigenvalue (to 32 eps |A|_F) exactly when A - (rho - 32 eps |A|_F) I is positive definite: no non-positive pivot.
+__device__ __forceinline__ bool eig9_nothing_below(const double* A, int r, int lane, double rho, double fro, double tiny,
+                                                   double* T) {
+  double a[9], ct[9], dinv;
+  return !eig9_factor_reg(A, r, lane, rho - 32.0 * 2.220446049250313e-16 * sqrt(fro), tiny, T, a, ct, dinv);
+}
+
 __device__ __noinline__ bool warp_smallest_eigvec9_reg(WarpScratch* ws, int lane) {
   const bool act = lane < 9;
   const int r = act ? lane : 0;            // idle lanes shadow row 0 (their values are never read)
@@ -270,6 +279,7 @@ __device__ __noinline__ bool warp_smallest_eigvec9_reg(WarpScratch* ws, int lane
   const double rr = s - rho * x;
   const double r2 = wl_sum(rr * rr);
   if (!(r2 <= 1e-28 * fro)) return false;
+  if (!eig9_nothing_below(A, r, lane, rho, fro, tiny, ws->aux)) return false;
   if (act) ws->cs[lane] = x;
   __syncwarp();
   return true;
@@ -337,7 +347,7 @@ __device__ __noinline__ bool warp_smallest_eigvec9_inv(WarpScratch* ws, int lane
   fro = wl_sum(act ? fro : 0.0);
   if (!((fro > 0.0) && (fro < 1e300))) return false;
   const double tiny = sqrt(fro) * 1e-30;
-  double m[9], x = 0.0;
+  double m[9], x = 0.0, mx2 = 0.0;         // mx2: |M x|^2 of the last step
   double sigma = 0.0, good = 0.0;
   bool need = true, have_x = false, done = false;
   int nfac = 0, allow_at = 1;
@@ -370,6 +380,7 @@ __device__ __noinline__ bool warp_smallest_eigvec9_inv(WarpScratch* ws, int lane
       dot += __shfl_xor_sync(0xffffffffu, dot, o);
     }
     if (!(n2 > 0.0) || !(n2 < 1e300)) return false;
+    mx2 = n2;
     const double xn = y * ((dot < 0.0 ? -1.0 : 1.0) * rsqrt(n2));
     const double df = xn - x;
     x = xn;
@@ -396,6 +407,12 @@ __device__ __noinline__ bool warp_smallest_eigvec9_inv(WarpScratch* ws, int lane
   const double rr = s - rho * x;
   const double r2 = wl_sum(rr * rr);
   if (!(r2 <= 1e-28 * fro)) return false;
+  // M = (A - good I)^-1 has the eigenvalues 1 / (lambda_i - good) > 0, so an x of a larger eigenvalue has
+  // trace(M) >= 2 |M x|: a well-separated lambda_min is settled here, the others by the inertia count
+  double tr = 0.0;
+#pragma unroll
+  for (int j = 0; j < 9; ++j) tr += shfl_d(m[j], j);
+  if (!(tr > 0.0 && tr * tr <= 1.5625 * mx2) && !eig9_nothing_below(A, r, lane, rho, fro, tiny, ws->aux)) return false;
   if (act) ws->cs[lane] = x;
   __syncwarp();
   return true;
