@@ -115,7 +115,11 @@ int dgb200_find_homography_ragged(const double* x1y1, const double* x2y2, const 
                                   double laf_coef, const uint64_t* seeds,
                                   double* H_out, uint8_t* mask_out, int32_t* stats_out);
 /* DEVICE-pointer flavour of the ragged batches (d_offsets in device memory; n_max = the largest pair, it sizes the
- * per-CTA scratch).  Asynchronous on `stream`. */
+ * per-CTA scratch).  Asynchronous on `stream`.  The device offsets are not read on the host (they may come from
+ * dgb200_match_descriptors_batch_dev), so the kernel guards every pair once: a pair with fewer than 8 (F) / 4 (H) rows,
+ * or more than n_max rows, is not run -- all-zero model, zero stats, its mask rows left as the caller initialised them
+ * (zero them first), no access past the pair's rows.  Offsets must start at 0 and stay within the arrays.  n_max itself
+ * must be >= 8 (F) / >= 4 (H). */
 int dgb200_find_fundamental_ragged_dev(const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets, int n_pairs,
                                        int n_max, int dim, double px_th, double conf, int max_iters, int error_type,
                                        int sym_check, double laf_coef, int degen_check, const uint64_t* d_seeds,
@@ -158,6 +162,29 @@ int dgb200_match_descriptors_dev(const float* d_desc1, int n1, const float* d_de
                                  const double* d_kp1, const double* d_kp2, int kp_dim, int* d_match_q, int* d_match_t,
                                  double* d_x1y1, double* d_x2y2, int out_dim, int capacity, int* d_count, void* d_workspace,
                                  void* stream);
+/* Descriptor matching of MANY image pairs in one call: the matcher above over a batch, with its output in the ragged
+ * layout that dgb200_find_*_ragged_dev take.
+ *   d_bank [R][D] float32: the descriptors of n_images images concatenated; image i owns rows
+ *          img_offsets[i] .. img_offsets[i+1]-1 (img_offsets: HOST int32 [n_images+1], starting at 0, non-decreasing).
+ *          Any 4-byte alignment (a 16-byte aligned bank is staged with bulk async copies).
+ *   pairs  HOST int32 [n_pairs][2] = (query image, train image); an image may appear in many pairs, on either side.
+ *   d_kp_bank [R][kp_dim] float64 or NULL: keypoint rows of the same images, gathered like dgb200_match_descriptors_dev.
+ * Output: pair p's matches, in ascending query order, are rows d_offsets_out[p] .. d_offsets_out[p+1]-1 of d_match_q,
+ * d_match_t (int32, indices local to each image) and, when d_x1y1 != NULL, of d_x1y1 / d_x2y2 [capacity][out_dim];
+ * d_offsets_out: DEVICE int32 [n_pairs+1], d_offsets_out[0] = 0.  capacity must be >= the sum over the pairs of the
+ * query image's descriptor count (every match of a pair is a distinct query); rows past d_offsets_out[n_pairs] are
+ * left unwritten.  A pair whose query image has no descriptors, or whose train image has fewer than 2, gets zero
+ * matches.  Malformed metadata (an image index out of range, decreasing offsets, D not a multiple of 4 in [4, 256],
+ * capacity too small) returns DGB200_E_ARG before anything is launched.  The image offsets and pair table are read on
+ * the host and copied (with the per-pair work layout derived from them) into d_workspace, sized by
+ * dgb200_match_batch_workspace_bytes() (0: malformed metadata).  Asynchronous on `stream`, no synchronisation; the
+ * host arrays may be freed on return.  Re-entrant: calls with distinct workspaces may run on different streams. */
+size_t dgb200_match_batch_workspace_bytes(const int32_t* img_offsets, int n_images, const int32_t* pairs, int n_pairs);
+int dgb200_match_descriptors_batch_dev(const float* d_bank, const int32_t* img_offsets, int n_images, int D,
+                                       const int32_t* pairs, int n_pairs, float ratio, int mutual, const double* d_kp_bank,
+                                       int kp_dim, int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
+                                       int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                       void* stream);
 /* Pose from fundamental matrices: E = K2^T F K1, the four (R, t) candidates of its SVD, cheirality vote over the
  * correspondences with mask != 0 (NULL: all).  d_K1/d_K2: one 3x3 (k_per_pair = 0) or one per pair, row-major.
  * Outputs R [n_pairs][9] row-major, t [n_pairs][3] (unit length, x2 ~ R x1 + t), good [n_pairs] = supporters or NULL.

@@ -50,6 +50,10 @@ def lib():
         L.dgb200_match_workspace_bytes.restype = ctypes.c_size_t
         L.dgb200_match_workspace_bytes.argtypes = [ci, ci]
         L.dgb200_match_descriptors_dev.argtypes = [vp, ci, vp, ci, ci, ctypes.c_float, ci, vp, vp, ci, vp, vp, vp, vp, ci, ci, vp, vp, vp]
+        L.dgb200_match_batch_workspace_bytes.restype = ctypes.c_size_t
+        L.dgb200_match_batch_workspace_bytes.argtypes = [i32, ci, i32, ci]
+        L.dgb200_match_descriptors_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, ctypes.c_float, ci, vp, ci, vp, vp, vp, vp,
+                                                         ci, ci, vp, vp, vp]
         L.dgb200_pose_from_fundamental_batch_dev.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p
@@ -192,6 +196,25 @@ def homography_batch_dev(d_p1, d_p2, P, N, dim, px_th, conf, max_iters, error_ty
     rc = lib().dgb200_find_homography_batch_dev_ex(d_p1, d_p2, P, N, dim, float(px_th), float(conf), int(max_iters),
                                                    int(error_type), int(bool(sym_check)), float(laf_coef), d_seeds, d_H,
                                                    d_mask, d_stats, stream, int(flags))
+    if rc != 0:
+        _raise(rc)
+
+
+def fundamental_ragged_dev(d_p1, d_p2, d_offsets, P, n_max, dim, px_th, conf, max_iters, error_type, sym_check, laf_coef,
+                           degen_check, d_seeds, d_F, d_mask, d_stats, stream=0):
+    """Device-pointer ragged batch: pair p owns rows d_offsets[p] .. d_offsets[p+1]-1 (int32 device array)."""
+    rc = lib().dgb200_find_fundamental_ragged_dev(d_p1, d_p2, d_offsets, P, int(n_max), dim, float(px_th), float(conf),
+                                                  int(max_iters), int(error_type), int(bool(sym_check)), float(laf_coef),
+                                                  int(bool(degen_check)), d_seeds, d_F, d_mask, d_stats, stream)
+    if rc != 0:
+        _raise(rc)
+
+
+def homography_ragged_dev(d_p1, d_p2, d_offsets, P, n_max, dim, px_th, conf, max_iters, error_type, sym_check, laf_coef,
+                          d_seeds, d_H, d_mask, d_stats, stream=0):
+    rc = lib().dgb200_find_homography_ragged_dev(d_p1, d_p2, d_offsets, P, int(n_max), dim, float(px_th), float(conf),
+                                                 int(max_iters), int(error_type), int(bool(sym_check)), float(laf_coef),
+                                                 d_seeds, d_H, d_mask, d_stats, stream)
     if rc != 0:
         _raise(rc)
 

@@ -162,6 +162,15 @@ __global__ void __launch_bounds__(kMaxThreads, DG_LB_BLOCKS) ransac_pairs_kernel
     // ---- stage the pair: HBM -> SoA tile (the only read of the pair from HBM)
     const size_t row0 = a.offsets ? (size_t)a.offsets[p] : (size_t)p * a.n;
     const int n = a.offsets ? a.offsets[p + 1] - a.offsets[p] : a.n;
+    if (a.offsets && (n < (KIND == 0 ? 8 : 4) || n > a.n)) {
+      // Ragged batches whose offsets were written on the device (a matcher, say) reach here unchecked: a pair too short
+      // for a minimal sample, or longer than the n_max that sized the slabs, is not run.  It gets the all-zero model and
+      // zero stats, and its mask rows stay as the caller initialised them.  (Block-uniform: every thread reads the same
+      // offsets.)
+      if (gtid < 9) a.model_out[(size_t)p * 9 + gtid] = 0.0;
+      if (a.stats_out && gtid < 4) a.stats_out[(size_t)p * 4 + gtid] = 0;
+      continue;
+    }
     c.N = n;
     const double* g1 = a.x1y1 + row0 * a.dim;
     const double* g2 = (KIND == 2) ? g1 + 5 : a.x2y2 + row0 * a.dim;   // u10 rows: (x', y', a', b', c', x, y, a, b, c)

@@ -14,6 +14,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include <vector>
+
 #include "../../include/degensac_b200.h"
 #include "common.h"
 #include "la.h"
@@ -64,44 +66,59 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                : "memory");
 }
 
+// One matcher work unit per image pair.  Built on the host from the image offsets and the pair table, copied to the
+// device with the call; entry n_pairs holds the totals.
+struct PairMeta {
+  int qrow, n1;     // query descriptors: rows qrow .. qrow+n1-1 of the query bank
+  int trow, n2;     // train descriptors: rows trow .. trow+n2-1 of the train bank
+  int tile0;        // first 2-NN work item: prefix of ceil(n1 / kTQ); a degenerate pair (n1 < 1 or n2 < 2) has none
+  int row0;         // first per-query slot (nn_idx / nn_d1 / nn_d2): prefix of n1, which is also the output capacity
+  int col0;         // first col_best slot: prefix of n2, so that a train image shared by several pairs keeps them apart
+  int pad;
+};
+
 struct MatchArgs {
-  const float* d1; const float* d2;   // [n1][D], [n2][D]
-  int n1, n2, D;
+  const float* qbank; const float* tbank;   // [rows][D]: the query and train descriptors of every pair
+  const PairMeta* meta;                     // [n_pairs + 1]
+  int n_pairs, D;
   int use_bulk;                       // train rows are 16-byte aligned: stage them with cp.async.bulk
   int mutual;                         // also track, per train descriptor, its nearest query (col_best)
   int* nn_idx; float* nn_d1; float* nn_d2;          // per query: nearest train index, squared distances of the two nearest
   unsigned long long* col_best;       // per train descriptor: (squared distance bits << 32 | query index), atomicMin
 };
 
-// Two nearest train descriptors of every query descriptor (squared L2 in FP32, accumulated in descriptor order).
-__global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
+// Two nearest train descriptors of the queries q0 .. q0+kTQ-1 of one pair (squared L2 in FP32, accumulated in
+// descriptor order; ties go to the lowest train index).  d1 [n1][D], d2 [n2][D]; nn_* and col_best are the pair's own
+// segments.  Called by all kMatchThreads threads of the CTA.
+__device__ __forceinline__ void nn2_tile(const float* d1, int n1, const float* d2, int n2, int D, int q0, int use_bulk,
+                                         int mutual, int* nn_idx, float* nn_d1, float* nn_d2,
+                                         unsigned long long* col_best) {
   extern __shared__ __align__(128) unsigned char msm[];
   __shared__ __align__(8) uint64_t bar[2];
-  const int D = a.D, qs = D + 4;                        // padded query row: conflict-free 128-bit reads across queries
+  const int qs = D + 4;                                 // padded query row: conflict-free 128-bit reads across queries
   float* tq = reinterpret_cast<float*>(msm);            // [kTQ][D + 4]
   float* tt = tq + kTQ * qs;                             // 2 stages x [kTT][D]
   const size_t stage_floats = (size_t)kTT * D;
   const int tid = threadIdx.x, q = tid & 31, g = tid >> 5;
-  const int q0 = blockIdx.x * kTQ;
   for (int i = tid; i < kTQ * D; i += kMatchThreads) {
     const int r = i / D, c = i % D;
-    tq[r * qs + c] = (q0 + r < a.n1) ? a.d1[(size_t)(q0 + r) * D + c] : 0.f;
+    tq[r * qs + c] = (q0 + r < n1) ? d1[(size_t)(q0 + r) * D + c] : 0.f;
   }
   if (tid == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   __syncthreads();
-  const int ntiles = (a.n2 + kTT - 1) / kTT;
+  const int ntiles = (n2 + kTT - 1) / kTT;
   auto issue = [&](int t) {          // stage tile t (one elected thread; or cooperative loads when unaligned)
-    const int rows = min(kTT, a.n2 - t * kTT);
+    const int rows = min(kTT, n2 - t * kTT);
     float* dst = tt + (size_t)(t & 1) * stage_floats;
-    if (a.use_bulk) {
+    if (use_bulk) {
       if (tid == 0) {
         const uint32_t bytes = (uint32_t)(rows * D * sizeof(float));
         mbar_expect_tx(&bar[t & 1], bytes);
-        bulk_g2s(dst, a.d2 + (size_t)t * kTT * D, bytes, &bar[t & 1]);
+        bulk_g2s(dst, d2 + (size_t)t * kTT * D, bytes, &bar[t & 1]);
       }
     } else {
-      const float* src = a.d2 + (size_t)t * kTT * D;
+      const float* src = d2 + (size_t)t * kTT * D;
       for (int i = tid; i < rows * D; i += kMatchThreads) dst[i] = src[i];
     }
   };
@@ -110,8 +127,8 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
   if (ntiles > 0) issue(0);
   for (int t = 0; t < ntiles; ++t) {
     if (t + 1 < ntiles) issue(t + 1);                 // next tile in flight behind this one's math
-    if (a.use_bulk) mbar_wait(&bar[t & 1], (uint32_t)((t >> 1) & 1)); else __syncthreads();
-    const int rows = min(kTT, a.n2 - t * kTT);
+    if (use_bulk) mbar_wait(&bar[t & 1], (uint32_t)((t >> 1) & 1)); else __syncthreads();
+    const int rows = min(kTT, n2 - t * kTT);
     const float* B = tt + (size_t)(t & 1) * stage_floats;
     const float* A = tq + q * qs;
     // this thread: train rows g*16 .. g*16+15 of the tile, four at a time (query chunk loaded once per four rows)
@@ -140,16 +157,16 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
           const int gj = t * kTT + j;
           if (s < b1 || (s == b1 && gj < i1)) { b2 = b1; b1 = s; i1 = gj; }
           else if (s < b2) b2 = s;
-          if (a.mutual) {
+          if (mutual) {
             // nearest QUERY of train descriptor gj among this warp's 32 queries, then one atomic per warp and row
-            unsigned long long key = (q0 + q < a.n1) ? (((unsigned long long)__float_as_uint(s) << 32) | (unsigned)(q0 + q))
-                                                      : 0xffffffffffffffffull;
+            unsigned long long key = (q0 + q < n1) ? (((unsigned long long)__float_as_uint(s) << 32) | (unsigned)(q0 + q))
+                                                    : 0xffffffffffffffffull;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
               const unsigned long long other = __shfl_xor_sync(0xffffffffu, key, o);
               key = other < key ? other : key;
             }
-            if (q == 0) atomicMin(a.col_best + gj, key);
+            if (q == 0) atomicMin(col_best + gj, key);
           }
         }
       }
@@ -162,7 +179,7 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
   int* mi = reinterpret_cast<int*>(m2 + kMatchThreads);
   m1[tid] = b1; m2[tid] = b2; mi[tid] = i1;
   __syncthreads();
-  if (g == 0 && q0 + q < a.n1) {
+  if (g == 0 && q0 + q < n1) {
     float c1 = INFINITY, c2 = INFINITY;
     int ci = -1;
     for (int gg = 0; gg < 4; ++gg) {
@@ -172,51 +189,131 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
       else if (x1 < c2) c2 = x1;
       if (x2 < c2) c2 = x2;
     }
-    a.nn_idx[q0 + q] = ci; a.nn_d1[q0 + q] = c1; a.nn_d2[q0 + q] = c2;
+    nn_idx[q0 + q] = ci; nn_d1[q0 + q] = c1; nn_d2[q0 + q] = c2;
   }
 }
 
-// SNN ratio test (+ mutual check) and ORDERED compaction of the accepted matches; gathers the keypoint coordinates
-// into the [N,2] float64 arrays the RANSAC entry points take.  One CTA (n1 is a few thousand).
-__global__ void __launch_bounds__(1024) select_kernel(int n1, const int* nn_idx, const float* nn_d1, const float* nn_d2,
-                                                      const unsigned long long* col_best, float ratio2, int mutual,
-                                                      const double* kp1, const double* kp2, int kp_dim, int* match_q,
-                                                      int* match_t, double* x1y1, double* x2y2, int out_dim, int cap,
-                                                      int* count) {
+// One flat grid over the (pair, kTQ-query tile) work items of the whole batch: CTA b finds its pair by binary search
+// over the tile prefix (the last pair whose first tile is <= b: pairs without tiles share their successor's prefix).
+__global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
+  const int b = blockIdx.x;
+  int lo = 0, hi = a.n_pairs - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (a.meta[mid].tile0 <= b) lo = mid; else hi = mid - 1;
+  }
+  const PairMeta m = a.meta[lo];
+  nn2_tile(a.qbank + (size_t)m.qrow * a.D, m.n1, a.tbank + (size_t)m.trow * a.D, m.n2, a.D, (b - m.tile0) * kTQ,
+           a.use_bulk, a.mutual, a.nn_idx + m.row0, a.nn_d1 + m.row0, a.nn_d2 + m.row0, a.col_best + m.col0);
+}
+
+constexpr int kSelThreads = 512;
+
+struct SelectArgs {
+  const PairMeta* meta;
+  const int* nn_idx; const float* nn_d1; const float* nn_d2;
+  const unsigned long long* col_best;
+  float ratio2; int mutual;
+  int* counts;                                  // [n_pairs] accepted matches per pair
+};
+
+// SNN ratio test (+ mutual check) of query q of the pair described by m; the accepted train index in *j
+__device__ __forceinline__ bool accept_match(const SelectArgs& a, const PairMeta& m, int q, int* j) {
+  *j = a.nn_idx[m.row0 + q];
+  bool ok = *j >= 0 && a.nn_d1[m.row0 + q] < a.ratio2 * a.nn_d2[m.row0 + q];   // d1 < ratio * d2 on L2 distances (simple-example.py:50)
+  if (ok && a.mutual) ok = (unsigned)(a.col_best[m.col0 + *j] & 0xffffffffu) == (unsigned)q;
+  return ok;
+}
+
+// one CTA per pair: how many of its queries pass
+__global__ void __launch_bounds__(kSelThreads) count_kernel(SelectArgs a) {
+  __shared__ int wsum[kSelThreads / 32];
+  const PairMeta m = a.meta[blockIdx.x];
+  const int tid = threadIdx.x;
+  int c = 0;
+  if (m.n1 >= 1 && m.n2 >= 2)                   // degenerate pairs were not matched: zero matches
+    for (int q = tid; q < m.n1; q += kSelThreads) { int j; c += accept_match(a, m, q, &j) ? 1 : 0; }
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if ((tid & 31) == 0) wsum[tid >> 5] = c;
+  __syncthreads();
+  if (tid == 0) {
+    int tot = 0;
+    for (int w = 0; w < kSelThreads / 32; ++w) tot += wsum[w];
+    a.counts[blockIdx.x] = tot;
+  }
+}
+
+// exclusive scan of the per-pair counts in one CTA: offsets[0] = 0, offsets[p+1] = offsets[p] + counts[p]; *count_out
+// (when given) = min(offsets[n_pairs], cap)
+__global__ void __launch_bounds__(1024) scan_kernel(const int* counts, int n_pairs, int* offsets, int cap, int* count_out) {
   __shared__ int wsum[32];
   __shared__ int base;
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  if (tid == 0) base = 0;
+  if (tid == 0) { base = 0; offsets[0] = 0; }
   __syncthreads();
-  for (int q0 = 0; q0 < n1; q0 += 1024) {
-    const int q = q0 + tid;
-    bool ok = false;
-    int j = -1;
-    if (q < n1) {
-      j = nn_idx[q];
-      ok = j >= 0 && nn_d1[q] < ratio2 * nn_d2[q];          // d1 < ratio * d2 on L2 distances (simple-example.py:50)
-      if (ok && mutual) ok = (unsigned)(col_best[j] & 0xffffffffu) == (unsigned)q;
+  for (int p0 = 0; p0 < n_pairs; p0 += 1024) {
+    const int p = p0 + tid;
+    const int v = p < n_pairs ? counts[p] : 0;
+    int x = v;                                   // inclusive scan within the warp
+    for (int o = 1; o < 32; o <<= 1) {
+      const int y = __shfl_up_sync(0xffffffffu, x, o);
+      if (lane >= o) x += y;
     }
-    const unsigned m = __ballot_sync(0xffffffffu, ok);
-    if (lane == 0) wsum[wid] = __popc(m);
+    if (lane == 31) wsum[wid] = x;
     __syncthreads();
     int off = base;
     for (int w = 0; w < wid; ++w) off += wsum[w];
-    off += __popc(m & ((1u << lane) - 1u));
-    if (ok && off < cap) {
-      match_q[off] = q; match_t[off] = j;
-      if (x1y1) {
-        for (int c = 0; c < out_dim; ++c) {
-          x1y1[(size_t)off * out_dim + c] = kp1[(size_t)q * kp_dim + c];
-          x2y2[(size_t)off * out_dim + c] = kp2[(size_t)j * kp_dim + c];
-        }
-      }
-    }
+    if (p < n_pairs) offsets[p + 1] = off + x;
     __syncthreads();
     if (tid == 0) { int tot = 0; for (int w = 0; w < 32; ++w) tot += wsum[w]; base += tot; }
     __syncthreads();
   }
-  if (tid == 0) *count = base < cap ? base : cap;
+  if (tid == 0 && count_out) *count_out = base < cap ? base : cap;
+}
+
+struct WriteArgs {
+  SelectArgs s;
+  const int* offsets;                          // [n_pairs + 1] from scan_kernel
+  const double* kq; const double* kt; int kp_dim;   // keypoint banks (rows like the descriptor banks) or nullptr
+  int* match_q; int* match_t; double* x1y1; double* x2y2; int out_dim, cap;
+};
+
+// one CTA per pair: ORDERED compaction of its accepted matches into rows offsets[p] .. offsets[p+1]-1 (ascending query
+// order), indices local to each image; gathers the keypoint coordinates into the float64 arrays the RANSAC entry
+// points take.  Rows at or past `cap` are not written.
+__global__ void __launch_bounds__(kSelThreads) write_kernel(WriteArgs a) {
+  __shared__ int wsum[kSelThreads / 32];
+  __shared__ int base;
+  const PairMeta m = a.s.meta[blockIdx.x];
+  if (m.n1 < 1 || m.n2 < 2) return;            // (block-uniform)
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  if (tid == 0) base = a.offsets[blockIdx.x];
+  __syncthreads();
+  for (int q0 = 0; q0 < m.n1; q0 += kSelThreads) {
+    const int q = q0 + tid;
+    int j = -1;
+    const bool ok = q < m.n1 && accept_match(a.s, m, q, &j);
+    const unsigned msk = __ballot_sync(0xffffffffu, ok);
+    if (lane == 0) wsum[wid] = __popc(msk);
+    __syncthreads();
+    int off = base;
+    for (int w = 0; w < wid; ++w) off += wsum[w];
+    off += __popc(msk & ((1u << lane) - 1u));
+    if (ok && off < a.cap) {
+      a.match_q[off] = q; a.match_t[off] = j;
+      if (a.x1y1) {
+        const double* k1 = a.kq + ((size_t)m.qrow + q) * a.kp_dim;
+        const double* k2 = a.kt + ((size_t)m.trow + j) * a.kp_dim;
+        for (int c = 0; c < a.out_dim; ++c) {
+          a.x1y1[(size_t)off * a.out_dim + c] = k1[c];
+          a.x2y2[(size_t)off * a.out_dim + c] = k2[c];
+        }
+      }
+    }
+    __syncthreads();
+    if (tid == 0) { int tot = 0; for (int w = 0; w < kSelThreads / 32; ++w) tot += wsum[w]; base += tot; }
+    __syncthreads();
+  }
 }
 
 // ------------------------------------------------------------------------------------------------ pose from F
@@ -365,6 +462,90 @@ __global__ void div_check_kernel(unsigned long long seed, long long count, unsig
   if (local) atomicAdd(bad, local);
 }
 
+// ------------------------------------------------------------------------------------------------ matcher, host side
+// Workspace of a batch: per-pair metadata, counts and (single-pair calls) offsets, then col_best [sum n2] and the
+// per-query 2-NN results [sum n1]; every segment 256-byte aligned.
+size_t match_ws_bytes(long long sum_n1, long long sum_n2, int n_pairs) {
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  return al(sizeof(PairMeta) * ((size_t)n_pairs + 1)) + 2 * al(sizeof(int) * ((size_t)n_pairs + 1)) +
+         al(sizeof(unsigned long long) * (size_t)sum_n2) + 3 * al(sizeof(int) * (size_t)sum_n1);
+}
+
+// Pair metadata from the image offsets of the query and train banks (equal for a batch over one bank) and the pair
+// table [n_pairs][2] = (query image, train image).  Rejects malformed input; meta[n_pairs] holds the totals.
+int build_meta(const int32_t* qoff, const int32_t* toff, int n_images, const int32_t* pairs, int n_pairs,
+               std::vector<PairMeta>* meta) {
+  if (!qoff || !toff || !pairs) return fail2(DGB200_E_ARG, "null image offsets or pair table");
+  if (n_images < 1 || n_pairs < 1) return fail2(DGB200_E_ARG, "need n_images >= 1 and n_pairs >= 1");
+  for (const int32_t* off : {qoff, toff}) {
+    if (off[0] != 0) return fail2(DGB200_E_ARG, "image offsets must start at 0");
+    for (int i = 0; i < n_images; ++i)
+      if (off[i + 1] < off[i]) return fail2(DGB200_E_ARG, "image offsets must be non-decreasing");
+  }
+  meta->assign((size_t)n_pairs + 1, PairMeta{});
+  long long tiles = 0, rows = 0, cols = 0;
+  for (int p = 0; p < n_pairs; ++p) {
+    const int qi = pairs[2 * p], ti = pairs[2 * p + 1];
+    if (qi < 0 || qi >= n_images || ti < 0 || ti >= n_images) return fail2(DGB200_E_ARG, "pair table: image index out of range");
+    PairMeta& m = (*meta)[p];
+    m.qrow = qoff[qi]; m.n1 = qoff[qi + 1] - qoff[qi];
+    m.trow = toff[ti]; m.n2 = toff[ti + 1] - toff[ti];
+    m.tile0 = (int)tiles; m.row0 = (int)rows; m.col0 = (int)cols;
+    if (m.n1 >= 1 && m.n2 >= 2) tiles += (m.n1 + kTQ - 1) / kTQ;   // degenerate pairs: no work, zero matches
+    rows += m.n1;
+    cols += m.n2;
+    if (rows > INT32_MAX || cols > INT32_MAX) return fail2(DGB200_E_ARG, "batch too large: more than 2^31 - 1 rows");
+  }
+  PairMeta& e = (*meta)[n_pairs];
+  e.tile0 = (int)tiles; e.row0 = (int)rows; e.col0 = (int)cols;
+  return 0;
+}
+
+// The matcher over a checked batch, asynchronous on st: metadata upload, 2-NN over all work items, per-pair counts,
+// scan, ordered write.  offsets == nullptr: a workspace segment holds them.
+int run_match(const float* qbank, const float* tbank, int D, const std::vector<PairMeta>& meta, float ratio, int mutual,
+              const double* kq, const double* kt, int kp_dim, int* match_q, int* match_t, double* x1y1, double* x2y2,
+              int out_dim, int cap, int* offsets, int* count_out, void* workspace, cudaStream_t st) {
+  const int P = (int)meta.size() - 1;
+  const PairMeta& tot = meta[P];
+  auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+  unsigned char* w = (unsigned char*)workspace;
+  PairMeta* d_meta = (PairMeta*)w; w += al(sizeof(PairMeta) * ((size_t)P + 1));
+  int* counts = (int*)w; w += al(sizeof(int) * ((size_t)P + 1));
+  int* ws_offsets = (int*)w; w += al(sizeof(int) * ((size_t)P + 1));
+  MatchArgs a;
+  a.col_best = (unsigned long long*)w; w += al(sizeof(unsigned long long) * (size_t)tot.col0);
+  a.nn_idx = (int*)w; w += al(sizeof(int) * (size_t)tot.row0);
+  a.nn_d1 = (float*)w; w += al(sizeof(float) * (size_t)tot.row0);
+  a.nn_d2 = (float*)w;
+  if (!offsets) offsets = ws_offsets;
+  a.qbank = qbank; a.tbank = tbank; a.meta = d_meta; a.n_pairs = P; a.D = D;
+  a.use_bulk = (((uintptr_t)tbank) & 15) == 0 ? 1 : 0;   // every image's rows then are too (D % 4 == 0)
+  a.mutual = mutual;
+  // pageable source: the runtime stages it before returning, the copy itself is ordered on st like the kernels
+  CU2(cudaMemcpyAsync(d_meta, meta.data(), sizeof(PairMeta) * meta.size(), cudaMemcpyHostToDevice, st));
+  if (tot.tile0 > 0) {
+    if (mutual) CU2(cudaMemsetAsync(a.col_best, 0xff, sizeof(unsigned long long) * (size_t)tot.col0, st));
+    const size_t smem = sizeof(float) * ((size_t)kTQ * (D + 4) + 2 * (size_t)kTT * D);
+    CU2(cudaFuncSetAttribute(nn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    nn2_kernel<<<tot.tile0, kMatchThreads, smem, st>>>(a);
+    CU2(cudaGetLastError());
+  }
+  SelectArgs s;
+  s.meta = d_meta; s.nn_idx = a.nn_idx; s.nn_d1 = a.nn_d1; s.nn_d2 = a.nn_d2; s.col_best = a.col_best;
+  s.ratio2 = ratio * ratio; s.mutual = mutual; s.counts = counts;
+  count_kernel<<<P, kSelThreads, 0, st>>>(s);
+  CU2(cudaGetLastError());
+  scan_kernel<<<1, 1024, 0, st>>>(counts, P, offsets, cap, count_out);
+  CU2(cudaGetLastError());
+  WriteArgs wa;
+  wa.s = s; wa.offsets = offsets; wa.kq = kq; wa.kt = kt; wa.kp_dim = kp_dim;
+  wa.match_q = match_q; wa.match_t = match_t; wa.x1y1 = x1y1; wa.x2y2 = x2y2; wa.out_dim = out_dim; wa.cap = cap;
+  write_kernel<<<P, kSelThreads, 0, st>>>(wa);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -383,7 +564,14 @@ int dgb200_debug_div_check(unsigned long long seed, long long count, unsigned lo
 const char* dgb200_frontend_last_error(void) { return g_err2; }
 
 size_t dgb200_match_workspace_bytes(int n1, int n2) {
-  return (size_t)n1 * (sizeof(int) + 2 * sizeof(float)) + (size_t)n2 * sizeof(unsigned long long) + 256;
+  if (n1 < 0 || n2 < 0) return 0;
+  return match_ws_bytes(n1, n2, 1);
+}
+
+size_t dgb200_match_batch_workspace_bytes(const int32_t* img_offsets, int n_images, const int32_t* pairs, int n_pairs) {
+  std::vector<PairMeta> meta;
+  if (build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta)) return 0;
+  return match_ws_bytes(meta[n_pairs].row0, meta[n_pairs].col0, n_pairs);
 }
 
 int dgb200_match_descriptors_dev(const float* d_desc1, int n1, const float* d_desc2, int n2, int D, float ratio, int mutual,
@@ -394,25 +582,30 @@ int dgb200_match_descriptors_dev(const float* d_desc1, int n1, const float* d_de
   if (n1 < 1 || n2 < 2) return fail2(DGB200_E_ARG, "need n1 >= 1 query and n2 >= 2 train descriptors");
   if (D < 4 || D > 256 || (D & 3)) return fail2(DGB200_E_ARG, "descriptor length must be a multiple of 4 in [4, 256]");
   if (d_x1y1 && (!d_kp1 || !d_kp2 || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
-  cudaStream_t st = (cudaStream_t)stream;
-  unsigned char* w = (unsigned char*)d_workspace;
-  MatchArgs a;
-  a.d1 = d_desc1; a.d2 = d_desc2; a.n1 = n1; a.n2 = n2; a.D = D;
-  a.col_best = (unsigned long long*)w; w += (size_t)n2 * sizeof(unsigned long long);
-  a.nn_idx = (int*)w; w += (size_t)n1 * sizeof(int);
-  a.nn_d1 = (float*)w; w += (size_t)n1 * sizeof(float);
-  a.nn_d2 = (float*)w;
-  a.use_bulk = (((uintptr_t)d_desc2) & 15) == 0 ? 1 : 0;       // rows are multiples of 16 bytes (D % 4 == 0)
-  a.mutual = mutual;
-  CU2(cudaMemsetAsync(a.col_best, 0xff, (size_t)n2 * sizeof(unsigned long long), st));
-  const size_t smem = sizeof(float) * ((size_t)kTQ * (D + 4) + 2 * (size_t)kTT * D);
-  CU2(cudaFuncSetAttribute(nn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  nn2_kernel<<<(n1 + kTQ - 1) / kTQ, kMatchThreads, smem, st>>>(a);
-  CU2(cudaGetLastError());
-  select_kernel<<<1, 1024, 0, st>>>(n1, a.nn_idx, a.nn_d1, a.nn_d2, a.col_best, ratio * ratio, mutual, d_kp1, d_kp2, kp_dim,
-                                    d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_count);
-  CU2(cudaGetLastError());
-  return 0;
+  // a batch of one pair: image 0 is the query image in the first bank, image 1 the train image in the second
+  const int32_t qoff[3] = {0, n1, n1}, toff[3] = {0, 0, n2}, pair[2] = {0, 1};
+  std::vector<PairMeta> meta;
+  const int rc = build_meta(qoff, toff, 2, pair, 1, &meta);
+  if (rc) return rc;
+  return run_match(d_desc1, d_desc2, D, meta, ratio, mutual, d_kp1, d_kp2, kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2,
+                   out_dim, capacity, nullptr, d_count, d_workspace, (cudaStream_t)stream);
+}
+
+int dgb200_match_descriptors_batch_dev(const float* d_bank, const int32_t* img_offsets, int n_images, int D,
+                                       const int32_t* pairs, int n_pairs, float ratio, int mutual, const double* d_kp_bank,
+                                       int kp_dim, int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
+                                       int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                       void* stream) {
+  if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
+  if (D < 4 || D > 256 || (D & 3)) return fail2(DGB200_E_ARG, "descriptor length must be a multiple of 4 in [4, 256]");
+  if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  std::vector<PairMeta> meta;
+  const int rc = build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta);
+  if (rc) return rc;
+  if (!d_bank && meta[n_pairs].tile0 > 0) return fail2(DGB200_E_ARG, "null descriptor bank");
+  if (capacity < meta[n_pairs].row0) return fail2(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
+  return run_match(d_bank, d_bank, D, meta, ratio, mutual, d_kp_bank, d_kp_bank, kp_dim, d_match_q, d_match_t, d_x1y1,
+                   d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream);
 }
 
 int dgb200_pose_from_fundamental_batch_dev(const double* d_F, const double* d_K1, const double* d_K2, int k_per_pair,

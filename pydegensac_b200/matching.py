@@ -7,10 +7,48 @@ descriptors go in, models and masks come out, nothing visits the host in between
 
     idx1, idx2, pts1, pts2 = match_descriptors(desc1, desc2, kp1, kp2, ratio=0.9)
     F, mask = pydegensac_b200.findFundamentalMatrixBatch(pts1[None], pts2[None], 0.5, 0.999, 50000)
+
+Many image pairs at once (one matcher call, one RANSAC launch, no host read in between):
+
+    m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
+    F, mask = pydegensac_b200.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, offsets=m.offsets,
+                                                         n_max=m.n_max)
 """
+import collections
 import ctypes
 
+import numpy as np
+
 from . import _cabi
+
+kTQ = 32   # query descriptors per 2-NN work item (frontend.cu)
+
+BatchLayout = collections.namedtuple("BatchLayout", "tile_prefix row_prefix col_prefix capacity n_max")
+BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offsets n_max")
+
+
+def batch_layout(counts, pairs):
+    """Work layout of a matcher batch, from the descriptor counts of the images and the [P,2] pair table
+    (query image, train image) -- what dgb200_match_descriptors_batch_dev derives on the host:
+    tile_prefix [P+1]: first 2-NN work item of each pair (ceil(n1/32) items; none for a pair whose query image has no
+    descriptors or whose train image has fewer than 2); row_prefix [P+1]: first output row a pair may use (prefix of the
+    query counts); col_prefix [P+1]: the pair's col_best segment (prefix of the train counts); capacity = row_prefix[P];
+    n_max = the largest query-image count over the pairs (an upper bound on any pair's match count)."""
+    c = np.asarray(counts, dtype=np.int64)
+    pr = np.asarray(pairs, dtype=np.int64)
+    if pr.ndim != 2 or pr.shape[1] != 2 or pr.shape[0] < 1:
+        raise ValueError("pairs must be a non-empty [P,2] array of (query image, train image)")
+    if pr.min() < 0 or pr.max() >= len(c):
+        raise ValueError("pairs: image index out of range")
+    n1, n2 = c[pr[:, 0]], c[pr[:, 1]]
+    tiles = np.where((n1 >= 1) & (n2 >= 2), (n1 + kTQ - 1) // kTQ, 0)
+
+    def prefix(x):
+        out = np.zeros(len(x) + 1, dtype=np.int64)
+        np.cumsum(x, out=out[1:])
+        return out
+    rows = prefix(n1)
+    return BatchLayout(prefix(tiles), rows, prefix(n2), int(rows[-1]), int(n1.max()))
 
 
 def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False):
@@ -97,3 +135,83 @@ def pose_from_fundamental(F, K1, K2, pts1, pts2, mask=None):
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return R, t, good
+
+
+def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False):
+    """match_descriptors over many image pairs in one call, output in the ragged layout of the offsets= entry points.
+
+    descs: list of I CUDA tensors [n_i, D] (n_i may be 0; converted to float32 like match_descriptors).
+    pairs: HOST [P,2] int array (numpy / list / CPU tensor) of (query image, train image); reading a CUDA tensor would
+    synchronise, so one is refused.  kps: optional list of I tensors [n_i, k] (k >= 2; six columns carry the local
+    affine shape through).
+    Returns BatchMatches(idx1, idx2, pts1, pts2, offsets, n_max): pair p's matches, in ascending query order, are rows
+    offsets[p] .. offsets[p+1]-1 of idx1/idx2 (int64, indices local to each image) and of pts1/pts2 (float64
+    [capacity, 2|6], None without kps); offsets is an int32 CUDA tensor [P+1]; n_max is a host int bounding every pair's
+    match count.  capacity is the sum of the query images' counts; rows past offsets[P] are unspecified.  A pair whose
+    query image is empty or whose train image has fewer than 2 descriptors has no matches.  Asynchronous: nothing is
+    read back from the device."""
+    import torch
+    if isinstance(pairs, torch.Tensor):
+        if pairs.is_cuda:
+            raise ValueError("pairs must be a host array: reading a CUDA tensor would synchronise")
+        pairs = pairs.numpy()
+    if len(descs) < 1:
+        raise ValueError("expected a non-empty list of descriptor tensors")
+    dev = descs[0].device
+    ds = [d.to(torch.float32) for d in descs]
+    if not dev.type == "cuda" or any(d.dim() != 2 or d.device != dev or d.shape[1] != ds[0].shape[1] for d in ds):
+        raise ValueError("expected CUDA descriptor tensors [n_i, D] with one D, on one device")
+    counts = [int(d.shape[0]) for d in ds]
+    bank = torch.cat(ds, 0).contiguous()
+    kbank = None
+    if kps is not None:
+        if len(kps) != len(ds):
+            raise ValueError("kps must hold one keypoint tensor per descriptor tensor")
+        ks = [k.to(device=dev, dtype=torch.float64) for k in kps]
+        if any(k.dim() != 2 or k.shape[0] != c or k.shape[1] != ks[0].shape[1] for k, c in zip(ks, counts)) \
+                or ks[0].shape[1] < 2:
+            raise ValueError("keypoint tensors must be [n_i, k] with one k >= 2")
+        kbank = torch.cat(ks, 0).contiguous()
+    return _match_bank(bank, counts, pairs, kbank, ratio, mutual)
+
+
+def _match_bank(bank, counts, pairs, kbank, ratio, mutual):
+    """The batched matcher over a descriptor bank [R,D] (any 4-byte alignment) whose image i owns rows
+    sum(counts[:i]) .. sum(counts[:i+1])-1; kbank: keypoint rows of the same images or None."""
+    import torch
+    pr = np.ascontiguousarray(np.asarray(pairs), dtype=np.int32)
+    lay = batch_layout(counts, pr)
+    off = np.zeros(len(counts) + 1, dtype=np.int32)
+    np.cumsum(counts, out=off[1:])
+    P = pr.shape[0]
+    D = int(bank.shape[1])
+    dev = bank.device
+    L = _cabi.lib()
+    i32 = ctypes.POINTER(ctypes.c_int32)
+    cap = max(lay.capacity, 1)        # (a zero-sized allocation would pass a null pointer)
+    with torch.cuda.device(dev):
+        mq = torch.empty(cap, dtype=torch.int32, device=dev)
+        mt = torch.empty(cap, dtype=torch.int32, device=dev)
+        offsets = torch.empty(P + 1, dtype=torch.int32, device=dev)
+        ws = torch.empty(max(int(L.dgb200_match_batch_workspace_bytes(off.ctypes.data_as(i32), len(counts),
+                                                                      pr.ctypes.data_as(i32), P)), 1),
+                         dtype=torch.uint8, device=dev)
+        x1 = x2 = None
+        kp_dim = out_dim = 0
+        if kbank is not None:
+            kp_dim = int(kbank.shape[1])
+            out_dim = 6 if kp_dim >= 6 else 2
+            x1 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
+            x2 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
+        stream = torch.cuda.current_stream(dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_match_descriptors_batch_dev(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D,
+                                                  pr.ctypes.data_as(i32), P, ctypes.c_float(ratio), int(bool(mutual)),
+                                                  vp(kbank.data_ptr()) if kbank is not None else None, kp_dim,
+                                                  vp(mq.data_ptr()), vp(mt.data_ptr()),
+                                                  vp(x1.data_ptr()) if x1 is not None else None,
+                                                  vp(x2.data_ptr()) if x2 is not None else None, out_dim, cap,
+                                                  vp(offsets.data_ptr()), vp(ws.data_ptr()), vp(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_frontend_last_error().decode())
+    return BatchMatches(mq.long(), mt.long(), x1, x2, offsets, lay.n_max)

@@ -92,12 +92,69 @@ def _launch(kind, p1, p2, px_th, conf, max_iters, et, sym, laf, degen, seeds, fl
     return model, mask, stats
 
 
+def _launch_ragged(kind, pts1, pts2, offsets, n_max, px_th, conf, max_iters, et, sym, laf_coef, degen, seeds, final_lsq):
+    """Ragged batch on the device: pts [rows, 2|6] CUDA tensors, pair p owns rows offsets[p] .. offsets[p+1]-1
+    (offsets: int32 CUDA tensor [P+1], e.g. from matching.match_descriptors_batch; n_max: a host int >= every pair's
+    length).  Nothing is read back: the kernel skips pairs that are too short or longer than n_max (zero model, False
+    mask rows, zero stats).  Returns (model [P,3,3], mask [rows] uint8, stats [P,4])."""
+    torch = _torch()
+    if final_lsq:
+        raise ValueError("final_lsq is not available with offsets=")
+    if n_max is None:
+        raise ValueError("offsets= needs n_max, the largest pair's row count (reading it from the device would synchronise)")
+    if not (isinstance(offsets, torch.Tensor) and offsets.is_cuda and offsets.dim() == 1 and offsets.shape[0] >= 2):
+        raise ValueError("offsets must be a CUDA tensor [P+1]")
+    p1 = pts1 if isinstance(pts1, torch.Tensor) else torch.from_dlpack(pts1)
+    p2 = pts2 if isinstance(pts2, torch.Tensor) else torch.from_dlpack(pts2)
+    if not p1.is_cuda or p1.dim() != 2 or p1.shape[1] not in (2, 6) or p1.shape != p2.shape or p1.device != p2.device \
+            or offsets.device != p1.device:
+        raise ValueError("with offsets=, pts1 and pts2 must be CUDA tensors [rows, 2] or [rows, 6] on the offsets' device")
+    p1, p2 = p1.to(torch.float64).contiguous(), p2.to(torch.float64).contiguous()
+    off = offsets.to(torch.int32).contiguous()
+    P = int(off.shape[0]) - 1
+    rows, dim = int(p1.shape[0]), int(p1.shape[1])
+    laf = _batch_laf(laf_coef, p1)
+    n_max = max(int(n_max), 8 if kind == 0 else 4)   # the slabs need room for one minimal sample; shorter pairs are skipped
+    dev = p1.device
+    with torch.cuda.device(dev):
+        _cabi.lib().dgb200_set_device(dev.index if dev.index is not None else torch.cuda.current_device())
+        model = torch.zeros((P, 3, 3), dtype=torch.float64, device=dev)
+        mask = torch.zeros(max(rows, 1), dtype=torch.uint8, device=dev)
+        stats = torch.zeros((P, 4), dtype=torch.int32, device=dev)
+        ds = _seeds_tensor(seeds, P, dev)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        args = (p1.data_ptr(), p2.data_ptr(), off.data_ptr(), P, n_max, dim, px_th, conf, max_iters, et, sym, laf)
+        if kind == 0:
+            _cabi.fundamental_ragged_dev(*args, degen, ds.data_ptr(), model.data_ptr(), mask.data_ptr(), stats.data_ptr(),
+                                         stream)
+        else:
+            _cabi.homography_ragged_dev(*args, ds.data_ptr(), model.data_ptr(), mask.data_ptr(), stats.data_ptr(), stream)
+    return model, mask[:rows], stats
+
+
+def _opencv_convention_nosync(Hraw):
+    """inv(H.T) per pair on the device without reading anything back: all-zero and singular models give all-zero H."""
+    torch = _torch()
+    Ht = Hraw.transpose(1, 2)
+    good = (Hraw.abs().sum(dim=(1, 2)) != 0) & (torch.linalg.det(Ht).abs() > 0)
+    eye = torch.eye(3, dtype=Hraw.dtype, device=Hraw.device).expand_as(Ht)
+    inv, _ = torch.linalg.inv_ex(torch.where(good[:, None, None], Ht, eye))
+    return torch.where(good[:, None, None], inv, torch.zeros_like(inv))
+
+
 def findFundamentalMatrixBatch(pts1, pts2, px_th=0.5, conf=0.9999, max_iters=100000, error_type="sampson",
                                symmetric_error_check=True, enable_degeneracy_check=True, seeds=None,
-                               return_stats=False, laf_consistensy_coef=-1.0, final_lsq=False):
+                               return_stats=False, laf_consistensy_coef=-1.0, final_lsq=False, offsets=None, n_max=None):
     """Device-resident batched findFundamentalMatrix: CUDA tensors in, CUDA tensors out
-    (F [P,3,3] float64, mask [P,N] bool[, stats [P,4] int32])."""
+    (F [P,3,3] float64, mask [P,N] bool[, stats [P,4] int32]).
+    offsets= (int32 CUDA [P+1]) with n_max: a ragged batch, pts [rows, 2|6] -> mask [rows] bool aligned with pts."""
     et = _error_type(error_type, error_type_dict_fundamental)
+    if offsets is not None:
+        F, mask, stats = _launch_ragged(0, pts1, pts2, offsets, n_max, float(px_th), float(conf), int(max_iters), et,
+                                        bool(symmetric_error_check), laf_consistensy_coef, bool(enable_degeneracy_check),
+                                        seeds, final_lsq)
+        mask = mask.view(_torch().bool)
+        return (F, mask, stats) if return_stats else (F, mask)
     p1, p2 = as_device_f64(pts1), as_device_f64(pts2)
     laf = _batch_laf(laf_consistensy_coef, p1)
     F, mask, stats = _launch(0, p1, p2, float(px_th), float(conf), int(max_iters), et, bool(symmetric_error_check), laf,
@@ -108,11 +165,18 @@ def findFundamentalMatrixBatch(pts1, pts2, px_th=0.5, conf=0.9999, max_iters=100
 
 def findHomographyBatch(pts1, pts2, px_th=1.0, conf=0.999, max_iters=50000, error_type="sampson",
                         symmetric_error_check=True, seeds=None, return_stats=False, laf_consistensy_coef=-1.0,
-                        final_lsq=False):
+                        final_lsq=False, offsets=None, n_max=None):
     """Device-resident batched findHomography: H [P,3,3] in the OpenCV convention (x2 ~ H x1; the core's raw
-    column-major image2->image1 model is inverted/transposed on the device, utils.py:108), mask [P,N] bool."""
+    column-major image2->image1 model is inverted/transposed on the device, utils.py:108), mask [P,N] bool.
+    offsets= (int32 CUDA [P+1]) with n_max: a ragged batch, pts [rows, 2|6] -> mask [rows] bool aligned with pts."""
     torch = _torch()
     et = _error_type(error_type, error_type_dict_homography)
+    if offsets is not None:
+        Hraw, mask, stats = _launch_ragged(1, pts1, pts2, offsets, n_max, float(px_th), float(conf), int(max_iters), et,
+                                           bool(symmetric_error_check), laf_consistensy_coef, False, seeds, final_lsq)
+        H = _opencv_convention_nosync(Hraw)
+        mask = mask.view(torch.bool)
+        return (H, mask, stats) if return_stats else (H, mask)
     p1, p2 = as_device_f64(pts1), as_device_f64(pts2)
     laf = _batch_laf(laf_consistensy_coef, p1)
     Hraw, mask, stats = _launch(1, p1, p2, float(px_th), float(conf), int(max_iters), et, bool(symmetric_error_check),

@@ -187,20 +187,25 @@ def _batch_laf(coef, p1):
 
 def findFundamentalMatrixBatch(pts1, pts2, px_th=0.5, conf=0.9999, max_iters=100000, error_type="sampson",
                                symmetric_error_check=True, enable_degeneracy_check=True, seeds=None,
-                               return_stats=False, laf_consistensy_coef=-1.0, final_lsq=False):
+                               return_stats=False, laf_consistensy_coef=-1.0, final_lsq=False, offsets=None, n_max=None):
     """Batched findFundamentalMatrix over P independent pairs: pts [P,N,2] (or [P,N,6] with local affine shapes)
     -> (F [P,3,3], mask [P,N] bool).  Pairs without a model get an all-zero F and an all-False mask row.
     RAGGED batches: pass two lists of [n_i, 2] (or [n_i, 6]) arrays -> (F [P,3,3], list of P bool masks); one kernel
     launch, same results as one call per pair with the same seed.
     CUDA tensors (torch, or any DLPack exporter) stay on the device: see pydegensac_b200.tensor_api.
-    final_lsq=True: the reference's compile-time __FINAL_LSQ__ polish (exp_ranF.c:1701-1705)."""
+    final_lsq=True: the reference's compile-time __FINAL_LSQ__ polish (exp_ranF.c:1701-1705).
+    offsets=, n_max=: a ragged batch resident on the device (tensor_api; CUDA tensors only), e.g. the output of
+    matching.match_descriptors_batch."""
     from . import _cabi
     if not isinstance(pts1, (np.ndarray, list, tuple)):
         from . import tensor_api
         if tensor_api.is_device_tensor(pts1):
             return tensor_api.findFundamentalMatrixBatch(pts1, pts2, px_th, conf, max_iters, error_type,
                                                          symmetric_error_check, enable_degeneracy_check, seeds,
-                                                         return_stats, laf_consistensy_coef, final_lsq)
+                                                         return_stats, laf_consistensy_coef, final_lsq,
+                                                         offsets=offsets, n_max=n_max)
+    if offsets is not None:
+        raise ValueError("offsets= takes CUDA tensors only")
     et = _error_type(error_type, error_type_dict_fundamental)
     if _is_ragged(pts1):
         F, masks, stats = _cabi.fundamental_ragged(pts1, pts2, px_th, conf, max_iters, et, symmetric_error_check,
@@ -217,16 +222,20 @@ def findFundamentalMatrixBatch(pts1, pts2, px_th=0.5, conf=0.9999, max_iters=100
 
 def findHomographyBatch(pts1, pts2, px_th=1.0, conf=0.999, max_iters=50000, error_type="sampson",
                         symmetric_error_check=True, seeds=None, return_stats=False, laf_consistensy_coef=-1.0,
-                        final_lsq=False):
+                        final_lsq=False, offsets=None, n_max=None):
     """Batched findHomography: pts [P,N,2] (or [P,N,6]) -> (H [P,3,3] OpenCV convention, mask [P,N] bool).
     RAGGED batches: two lists of [n_i, 2] (or [n_i, 6]) arrays -> (H [P,3,3], list of P bool masks).
-    CUDA tensors stay on the device (pydegensac_b200.tensor_api); final_lsq: __FINAL_LSQ__ (exp_ranH.c:866-870)."""
+    CUDA tensors stay on the device (pydegensac_b200.tensor_api); final_lsq: __FINAL_LSQ__ (exp_ranH.c:866-870).
+    offsets=, n_max=: a ragged batch resident on the device (CUDA tensors only)."""
     from . import _cabi
     if not isinstance(pts1, (np.ndarray, list, tuple)):
         from . import tensor_api
         if tensor_api.is_device_tensor(pts1):
             return tensor_api.findHomographyBatch(pts1, pts2, px_th, conf, max_iters, error_type, symmetric_error_check,
-                                                  seeds, return_stats, laf_consistensy_coef, final_lsq)
+                                                  seeds, return_stats, laf_consistensy_coef, final_lsq,
+                                                  offsets=offsets, n_max=n_max)
+    if offsets is not None:
+        raise ValueError("offsets= takes CUDA tensors only")
     et = _error_type(error_type, error_type_dict_homography)
     if _is_ragged(pts1):
         Hraw, masks, stats = _cabi.homography_ragged(pts1, pts2, px_th, conf, max_iters, et, symmetric_error_check,
