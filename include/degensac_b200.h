@@ -185,6 +185,24 @@ int dgb200_match_descriptors_batch_dev(const float* d_bank, const int32_t* img_o
                                        int kp_dim, int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
                                        int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
                                        void* stream);
+/* Binary descriptors (ORB, AKAZE/MLDB, BRISK, FREAK) by Hamming distance: what cv2.BFMatcher(cv2.NORM_HAMMING)
+ * .knnMatch(k=2) + `m.distance < ratio * n.distance` computes.  Each descriptor is a row of n_words 32-bit words
+ * (n_words a multiple of 4 in [4, 64]: up to 2048 bits; zero-pad shorter codes, which changes no distance); the distance
+ * is the number of differing bits.  Ties at the nearest distance go to the lowest train index, and d2 is the
+ * second-smallest distance of the multiset, so two trains tied at the minimum give d2 == d1.  A query is accepted when
+ * (double)d1 < ratio * (double)d2 (never on a tie when ratio <= 1); the mutual check is the float matcher's.  Every
+ * other argument, the output and the errors are those of the float twin above (malformed input, including n_words
+ * outside the allowed set, returns DGB200_E_ARG before any launch).  The workspace does not depend on the descriptor
+ * type: dgb200_match_workspace_bytes / dgb200_match_batch_workspace_bytes size it. */
+int dgb200_match_binary_descriptors_dev(const uint32_t* d_desc1, int n1, const uint32_t* d_desc2, int n2, int n_words,
+                                        double ratio, int mutual, const double* d_kp1, const double* d_kp2, int kp_dim,
+                                        int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim,
+                                        int capacity, int* d_count, void* d_workspace, void* stream);
+int dgb200_match_binary_descriptors_batch_dev(const uint32_t* d_bank, const int32_t* img_offsets, int n_images,
+                                              int n_words, const int32_t* pairs, int n_pairs, double ratio, int mutual,
+                                              const double* d_kp_bank, int kp_dim, int* d_match_q, int* d_match_t,
+                                              double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
+                                              int32_t* d_offsets_out, void* d_workspace, void* stream);
 /* Pose from fundamental matrices: E = K2^T F K1, the four (R, t) candidates of its SVD, cheirality vote over the
  * correspondences with mask != 0 (NULL: all).  d_K1/d_K2: one 3x3 (k_per_pair = 0) or one per pair, row-major.
  * Outputs R [n_pairs][9] row-major, t [n_pairs][3] (unit length, x2 ~ R x1 + t), good [n_pairs] = supporters or NULL.

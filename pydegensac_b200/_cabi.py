@@ -54,6 +54,10 @@ def lib():
         L.dgb200_match_batch_workspace_bytes.argtypes = [i32, ci, i32, ci]
         L.dgb200_match_descriptors_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, ctypes.c_float, ci, vp, ci, vp, vp, vp, vp,
                                                          ci, ci, vp, vp, vp]
+        L.dgb200_match_binary_descriptors_dev.argtypes = [vp, ci, vp, ci, ci, cd, ci, vp, vp, ci, vp, vp, vp, vp, ci, ci, vp,
+                                                          vp, vp]
+        L.dgb200_match_binary_descriptors_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, cd, ci, vp, ci, vp, vp, vp, vp,
+                                                                ci, ci, vp, vp, vp]
         L.dgb200_pose_from_fundamental_batch_dev.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p

@@ -3,7 +3,9 @@
 //   BEFORE  descriptor matching: brute-force L2 two-nearest-neighbour search + SNN ratio test (+ optional mutual
 //           check) producing the [N,2] correspondence arrays the RANSAC kernel consumes -- what the reference's
 //           pipeline does on the host with cv2.BFMatcher.knnMatch(k=2) and `m.distance < 0.9 * n.distance`
-//           (examples/simple-example.py:46-53), so that src_pts/dst_pts never visit the host.
+//           (examples/simple-example.py:46-53), so that src_pts/dst_pts never visit the host.  Binary descriptors
+//           (ORB, AKAZE, BRISK, FREAK) take the same path with the Hamming distance (cv2.NORM_HAMMING): one XOR and one
+//           POPC per 32 bits in place of the FP32 FMAs.
 //           The train descriptors are streamed through shared memory with Hopper BULK ASYNC COPIES
 //           (cp.async.bulk global->shared, completion on an mbarrier; UBLKCP in SASS), double buffered behind the math.
 //   AFTER   pose from a fundamental matrix: E = K2^T F K1, the four (R, t) candidates, cheirality vote over the
@@ -78,31 +80,78 @@ struct PairMeta {
 };
 
 struct MatchArgs {
-  const float* qbank; const float* tbank;   // [rows][D]: the query and train descriptors of every pair
+  const float* qbank; const float* tbank;   // [rows][D]: the query and train descriptors of every pair (binary rows:
+                                            // 32-bit words, read through Dist::Elem)
   const PairMeta* meta;                     // [n_pairs + 1]
   int n_pairs, D;
   int use_bulk;                       // train rows are 16-byte aligned: stage them with cp.async.bulk
   int mutual;                         // also track, per train descriptor, its nearest query (col_best)
-  int* nn_idx; float* nn_d1; float* nn_d2;          // per query: nearest train index, squared distances of the two nearest
-  unsigned long long* col_best;       // per train descriptor: (squared distance bits << 32 | query index), atomicMin
+  int* nn_idx; float* nn_d1; float* nn_d2;          // per query: nearest train index, distances of the two nearest
+  unsigned long long* col_best;       // per train descriptor: (distance bits << 32 | query index), atomicMin
 };
 
-// Two nearest train descriptors of the queries q0 .. q0+kTQ-1 of one pair (squared L2 in FP32, accumulated in
-// descriptor order; ties go to the lowest train index).  d1 [n1][D], d2 [n2][D]; nn_* and col_best are the pair's own
-// segments.  Called by all kMatchThreads threads of the CTA.
-__device__ __forceinline__ void nn2_tile(const float* d1, int n1, const float* d2, int n2, int D, int q0, int use_bulk,
-                                         int mutual, int* nn_idx, float* nn_d1, float* nn_d2,
-                                         unsigned long long* col_best) {
+// The distances of the matcher.  Each has a 4-byte element, reads rows 16 bytes at a time and accumulates four train
+// rows against one query row; key() maps a distance to 32 bits that order like it (the high word of col_best).
+// The distance is kept as a float in nn_d1 / nn_d2 and in the selection: exact for Hamming, which is <= 2048.
+struct L2Dist {             // squared L2 over float rows, FP32, accumulated in descriptor order
+  using Elem = float;
+  using Acc = float;
+  __device__ __forceinline__ static void acc4(const float* A, const float* B0, int r1, int r2, int r3, int D, float& s0,
+                                              float& s1, float& s2, float& s3) {
+    for (int k = 0; k < D; k += 4) {
+      const float4 av = *reinterpret_cast<const float4*>(A + k);
+      const float4 v0 = *reinterpret_cast<const float4*>(B0 + k);
+      const float4 v1 = *reinterpret_cast<const float4*>(B0 + (size_t)r1 * D + k);
+      const float4 v2 = *reinterpret_cast<const float4*>(B0 + (size_t)r2 * D + k);
+      const float4 v3 = *reinterpret_cast<const float4*>(B0 + (size_t)r3 * D + k);
+      float d;
+      d = av.x - v0.x; s0 = fmaf(d, d, s0); d = av.y - v0.y; s0 = fmaf(d, d, s0); d = av.z - v0.z; s0 = fmaf(d, d, s0); d = av.w - v0.w; s0 = fmaf(d, d, s0);
+      d = av.x - v1.x; s1 = fmaf(d, d, s1); d = av.y - v1.y; s1 = fmaf(d, d, s1); d = av.z - v1.z; s1 = fmaf(d, d, s1); d = av.w - v1.w; s1 = fmaf(d, d, s1);
+      d = av.x - v2.x; s2 = fmaf(d, d, s2); d = av.y - v2.y; s2 = fmaf(d, d, s2); d = av.z - v2.z; s2 = fmaf(d, d, s2); d = av.w - v2.w; s2 = fmaf(d, d, s2);
+      d = av.x - v3.x; s3 = fmaf(d, d, s3); d = av.y - v3.y; s3 = fmaf(d, d, s3); d = av.z - v3.z; s3 = fmaf(d, d, s3); d = av.w - v3.w; s3 = fmaf(d, d, s3);
+    }
+  }
+  __device__ __forceinline__ static uint32_t key(float s) { return __float_as_uint(s); }   // s >= 0
+};
+struct HammingDist {        // differing bits of binary rows of 32-bit words: one XOR and one POPC per word
+  using Elem = uint32_t;
+  using Acc = uint32_t;
+  __device__ __forceinline__ static void acc4(const uint32_t* A, const uint32_t* B0, int r1, int r2, int r3, int D,
+                                              uint32_t& s0, uint32_t& s1, uint32_t& s2, uint32_t& s3) {
+    for (int k = 0; k < D; k += 4) {
+      const uint4 av = *reinterpret_cast<const uint4*>(A + k);
+      const uint4 v0 = *reinterpret_cast<const uint4*>(B0 + k);
+      const uint4 v1 = *reinterpret_cast<const uint4*>(B0 + (size_t)r1 * D + k);
+      const uint4 v2 = *reinterpret_cast<const uint4*>(B0 + (size_t)r2 * D + k);
+      const uint4 v3 = *reinterpret_cast<const uint4*>(B0 + (size_t)r3 * D + k);
+      s0 += __popc(av.x ^ v0.x) + __popc(av.y ^ v0.y) + __popc(av.z ^ v0.z) + __popc(av.w ^ v0.w);
+      s1 += __popc(av.x ^ v1.x) + __popc(av.y ^ v1.y) + __popc(av.z ^ v1.z) + __popc(av.w ^ v1.w);
+      s2 += __popc(av.x ^ v2.x) + __popc(av.y ^ v2.y) + __popc(av.z ^ v2.z) + __popc(av.w ^ v2.w);
+      s3 += __popc(av.x ^ v3.x) + __popc(av.y ^ v3.y) + __popc(av.z ^ v3.z) + __popc(av.w ^ v3.w);
+    }
+  }
+  __device__ __forceinline__ static uint32_t key(uint32_t s) { return s; }
+};
+
+// Two nearest train descriptors of the queries q0 .. q0+kTQ-1 of one pair under the distance Dist (ties go to the
+// lowest train index).  d1 [n1][D], d2 [n2][D] elements; nn_* and col_best are the pair's own segments.  Called by all
+// kMatchThreads threads of the CTA.
+template <class Dist>
+__device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, const typename Dist::Elem* d2, int n2,
+                                         int D, int q0, int use_bulk, int mutual, int* nn_idx, float* nn_d1,
+                                         float* nn_d2, unsigned long long* col_best) {
+  using T = typename Dist::Elem;
+  using Acc = typename Dist::Acc;
   extern __shared__ __align__(128) unsigned char msm[];
   __shared__ __align__(8) uint64_t bar[2];
   const int qs = D + 4;                                 // padded query row: conflict-free 128-bit reads across queries
-  float* tq = reinterpret_cast<float*>(msm);            // [kTQ][D + 4]
-  float* tt = tq + kTQ * qs;                             // 2 stages x [kTT][D]
-  const size_t stage_floats = (size_t)kTT * D;
+  T* tq = reinterpret_cast<T*>(msm);                    // [kTQ][D + 4]
+  T* tt = tq + kTQ * qs;                                // 2 stages x [kTT][D]
+  const size_t stage_elems = (size_t)kTT * D;
   const int tid = threadIdx.x, q = tid & 31, g = tid >> 5;
   for (int i = tid; i < kTQ * D; i += kMatchThreads) {
     const int r = i / D, c = i % D;
-    tq[r * qs + c] = (q0 + r < n1) ? d1[(size_t)(q0 + r) * D + c] : 0.f;
+    tq[r * qs + c] = (q0 + r < n1) ? d1[(size_t)(q0 + r) * D + c] : T(0);
   }
   if (tid == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -110,15 +159,15 @@ __device__ __forceinline__ void nn2_tile(const float* d1, int n1, const float* d
   const int ntiles = (n2 + kTT - 1) / kTT;
   auto issue = [&](int t) {          // stage tile t (one elected thread; or cooperative loads when unaligned)
     const int rows = min(kTT, n2 - t * kTT);
-    float* dst = tt + (size_t)(t & 1) * stage_floats;
+    T* dst = tt + (size_t)(t & 1) * stage_elems;
     if (use_bulk) {
       if (tid == 0) {
-        const uint32_t bytes = (uint32_t)(rows * D * sizeof(float));
+        const uint32_t bytes = (uint32_t)(rows * D * sizeof(T));
         mbar_expect_tx(&bar[t & 1], bytes);
         bulk_g2s(dst, d2 + (size_t)t * kTT * D, bytes, &bar[t & 1]);
       }
     } else {
-      const float* src = d2 + (size_t)t * kTT * D;
+      const T* src = d2 + (size_t)t * kTT * D;
       for (int i = tid; i < rows * D; i += kMatchThreads) dst[i] = src[i];
     }
   };
@@ -129,37 +178,26 @@ __device__ __forceinline__ void nn2_tile(const float* d1, int n1, const float* d
     if (t + 1 < ntiles) issue(t + 1);                 // next tile in flight behind this one's math
     if (use_bulk) mbar_wait(&bar[t & 1], (uint32_t)((t >> 1) & 1)); else __syncthreads();
     const int rows = min(kTT, n2 - t * kTT);
-    const float* B = tt + (size_t)(t & 1) * stage_floats;
-    const float* A = tq + q * qs;
+    const T* B = tt + (size_t)(t & 1) * stage_elems;
+    const T* A = tq + q * qs;
     // this thread: train rows g*16 .. g*16+15 of the tile, four at a time (query chunk loaded once per four rows)
     for (int jb = g * 16; jb < g * 16 + 16 && jb < rows; jb += 4) {
-      float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
-      const float* B0 = B + (size_t)jb * D;
+      Acc s0 = 0, s1 = 0, s2 = 0, s3 = 0;
+      const T* B0 = B + (size_t)jb * D;
       const int r1 = (jb + 1 < rows) ? 1 : 0, r2 = (jb + 2 < rows) ? 2 : 0, r3 = (jb + 3 < rows) ? 3 : 0;
-      for (int k = 0; k < D; k += 4) {
-        const float4 av = *reinterpret_cast<const float4*>(A + k);
-        const float4 v0 = *reinterpret_cast<const float4*>(B0 + k);
-        const float4 v1 = *reinterpret_cast<const float4*>(B0 + (size_t)r1 * D + k);
-        const float4 v2 = *reinterpret_cast<const float4*>(B0 + (size_t)r2 * D + k);
-        const float4 v3 = *reinterpret_cast<const float4*>(B0 + (size_t)r3 * D + k);
-        float d;
-        d = av.x - v0.x; s0 = fmaf(d, d, s0); d = av.y - v0.y; s0 = fmaf(d, d, s0); d = av.z - v0.z; s0 = fmaf(d, d, s0); d = av.w - v0.w; s0 = fmaf(d, d, s0);
-        d = av.x - v1.x; s1 = fmaf(d, d, s1); d = av.y - v1.y; s1 = fmaf(d, d, s1); d = av.z - v1.z; s1 = fmaf(d, d, s1); d = av.w - v1.w; s1 = fmaf(d, d, s1);
-        d = av.x - v2.x; s2 = fmaf(d, d, s2); d = av.y - v2.y; s2 = fmaf(d, d, s2); d = av.z - v2.z; s2 = fmaf(d, d, s2); d = av.w - v2.w; s2 = fmaf(d, d, s2);
-        d = av.x - v3.x; s3 = fmaf(d, d, s3); d = av.y - v3.y; s3 = fmaf(d, d, s3); d = av.z - v3.z; s3 = fmaf(d, d, s3); d = av.w - v3.w; s3 = fmaf(d, d, s3);
-      }
-      const float sv[4] = {s0, s1, s2, s3};
+      Dist::acc4(A, B0, r1, r2, r3, D, s0, s1, s2, s3);
+      const Acc sv[4] = {s0, s1, s2, s3};
 #pragma unroll
       for (int u = 0; u < 4; ++u) {
         const int j = jb + u;
         if (j < rows) {                                // (warp-uniform: g and rows are)
-          const float s = sv[u];
+          const float s = (float)sv[u];
           const int gj = t * kTT + j;
           if (s < b1 || (s == b1 && gj < i1)) { b2 = b1; b1 = s; i1 = gj; }
           else if (s < b2) b2 = s;
           if (mutual) {
             // nearest QUERY of train descriptor gj among this warp's 32 queries, then one atomic per warp and row
-            unsigned long long key = (q0 + q < n1) ? (((unsigned long long)__float_as_uint(s) << 32) | (unsigned)(q0 + q))
+            unsigned long long key = (q0 + q < n1) ? (((unsigned long long)Dist::key(sv[u]) << 32) | (unsigned)(q0 + q))
                                                     : 0xffffffffffffffffull;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
@@ -195,7 +233,9 @@ __device__ __forceinline__ void nn2_tile(const float* d1, int n1, const float* d
 
 // One flat grid over the (pair, kTQ-query tile) work items of the whole batch: CTA b finds its pair by binary search
 // over the tile prefix (the last pair whose first tile is <= b: pairs without tiles share their successor's prefix).
+template <class Dist>
 __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
+  using T = typename Dist::Elem;
   const int b = blockIdx.x;
   int lo = 0, hi = a.n_pairs - 1;
   while (lo < hi) {
@@ -203,8 +243,9 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
     if (a.meta[mid].tile0 <= b) lo = mid; else hi = mid - 1;
   }
   const PairMeta m = a.meta[lo];
-  nn2_tile(a.qbank + (size_t)m.qrow * a.D, m.n1, a.tbank + (size_t)m.trow * a.D, m.n2, a.D, (b - m.tile0) * kTQ,
-           a.use_bulk, a.mutual, a.nn_idx + m.row0, a.nn_d1 + m.row0, a.nn_d2 + m.row0, a.col_best + m.col0);
+  nn2_tile<Dist>((const T*)(a.qbank + (size_t)m.qrow * a.D), m.n1, (const T*)(a.tbank + (size_t)m.trow * a.D), m.n2, a.D,
+                 (b - m.tile0) * kTQ, a.use_bulk, a.mutual, a.nn_idx + m.row0, a.nn_d1 + m.row0, a.nn_d2 + m.row0,
+                 a.col_best + m.col0);
 }
 
 constexpr int kSelThreads = 512;
@@ -214,13 +255,20 @@ struct SelectArgs {
   const int* nn_idx; const float* nn_d1; const float* nn_d2;
   const unsigned long long* col_best;
   float ratio2; int mutual;
+  int hamming; double ratio;                    // integer distances: the ratio test in FP64 on the distances themselves
   int* counts;                                  // [n_pairs] accepted matches per pair
 };
 
 // SNN ratio test (+ mutual check) of query q of the pair described by m; the accepted train index in *j
 __device__ __forceinline__ bool accept_match(const SelectArgs& a, const PairMeta& m, int q, int* j) {
   *j = a.nn_idx[m.row0 + q];
-  bool ok = *j >= 0 && a.nn_d1[m.row0 + q] < a.ratio2 * a.nn_d2[m.row0 + q];   // d1 < ratio * d2 on L2 distances (simple-example.py:50)
+  bool ok = *j >= 0;
+  if (ok) {
+    // d1 < ratio * d2 on the distances (simple-example.py:50): squared L2 against ratio^2 in FP32; Hamming distances
+    // exactly as the example evaluates them on cv2's, in double
+    const float d1 = a.nn_d1[m.row0 + q], d2 = a.nn_d2[m.row0 + q];
+    ok = a.hamming ? (double)d1 < a.ratio * (double)d2 : d1 < a.ratio2 * d2;
+  }
   if (ok && a.mutual) ok = (unsigned)(a.col_best[m.col0 + *j] & 0xffffffffu) == (unsigned)q;
   return ok;
 }
@@ -502,10 +550,11 @@ int build_meta(const int32_t* qoff, const int32_t* toff, int n_images, const int
 }
 
 // The matcher over a checked batch, asynchronous on st: metadata upload, 2-NN over all work items, per-pair counts,
-// scan, ordered write.  offsets == nullptr: a workspace segment holds them.
-int run_match(const float* qbank, const float* tbank, int D, const std::vector<PairMeta>& meta, float ratio, int mutual,
-              const double* kq, const double* kt, int kp_dim, int* match_q, int* match_t, double* x1y1, double* x2y2,
-              int out_dim, int cap, int* offsets, int* count_out, void* workspace, cudaStream_t st) {
+// scan, ordered write.  The banks hold float rows of D floats (squared L2; ratio is a float's value) or, when
+// `hamming`, binary rows of D 32-bit words.  offsets == nullptr: a workspace segment holds them.
+int run_match(const void* qbank, const void* tbank, int D, int hamming, const std::vector<PairMeta>& meta, double ratio,
+              int mutual, const double* kq, const double* kt, int kp_dim, int* match_q, int* match_t, double* x1y1,
+              double* x2y2, int out_dim, int cap, int* offsets, int* count_out, void* workspace, cudaStream_t st) {
   const int P = (int)meta.size() - 1;
   const PairMeta& tot = meta[P];
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -519,21 +568,24 @@ int run_match(const float* qbank, const float* tbank, int D, const std::vector<P
   a.nn_d1 = (float*)w; w += al(sizeof(float) * (size_t)tot.row0);
   a.nn_d2 = (float*)w;
   if (!offsets) offsets = ws_offsets;
-  a.qbank = qbank; a.tbank = tbank; a.meta = d_meta; a.n_pairs = P; a.D = D;
+  a.qbank = (const float*)qbank; a.tbank = (const float*)tbank; a.meta = d_meta; a.n_pairs = P; a.D = D;
   a.use_bulk = (((uintptr_t)tbank) & 15) == 0 ? 1 : 0;   // every image's rows then are too (D % 4 == 0)
   a.mutual = mutual;
   // pageable source: the runtime stages it before returning, the copy itself is ordered on st like the kernels
   CU2(cudaMemcpyAsync(d_meta, meta.data(), sizeof(PairMeta) * meta.size(), cudaMemcpyHostToDevice, st));
   if (tot.tile0 > 0) {
     if (mutual) CU2(cudaMemsetAsync(a.col_best, 0xff, sizeof(unsigned long long) * (size_t)tot.col0, st));
+    // (both element types are 4 bytes)
     const size_t smem = sizeof(float) * ((size_t)kTQ * (D + 4) + 2 * (size_t)kTT * D);
-    CU2(cudaFuncSetAttribute(nn2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    nn2_kernel<<<tot.tile0, kMatchThreads, smem, st>>>(a);
+    void (*kern)(MatchArgs) = hamming ? nn2_kernel<HammingDist> : nn2_kernel<L2Dist>;
+    CU2(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kern<<<tot.tile0, kMatchThreads, smem, st>>>(a);
     CU2(cudaGetLastError());
   }
   SelectArgs s;
   s.meta = d_meta; s.nn_idx = a.nn_idx; s.nn_d1 = a.nn_d1; s.nn_d2 = a.nn_d2; s.col_best = a.col_best;
-  s.ratio2 = ratio * ratio; s.mutual = mutual; s.counts = counts;
+  s.ratio2 = (float)ratio * (float)ratio; s.mutual = mutual; s.counts = counts;
+  s.hamming = hamming; s.ratio = ratio;
   count_kernel<<<P, kSelThreads, 0, st>>>(s);
   CU2(cudaGetLastError());
   scan_kernel<<<1, 1024, 0, st>>>(counts, P, offsets, cap, count_out);
@@ -544,6 +596,50 @@ int run_match(const float* qbank, const float* tbank, int D, const std::vector<P
   write_kernel<<<P, kSelThreads, 0, st>>>(wa);
   CU2(cudaGetLastError());
   return 0;
+}
+
+// Row lengths: float rows of D floats, binary rows of n_words 32-bit words.  The error message, or nullptr when valid.
+const char* float_len_error(int D) {
+  return (D < 4 || D > 256 || (D & 3)) ? "descriptor length must be a multiple of 4 in [4, 256]" : nullptr;
+}
+const char* word_len_error(int n_words) {
+  return (n_words < 4 || n_words > 64 || (n_words & 3)) ? "binary descriptor length must be a multiple of 4 in [4, 64] words"
+                                                        : nullptr;
+}
+
+// One pair (dgb200_match_descriptors_dev and its binary twin): a batch of one pair, image 0 the query image in the
+// first bank, image 1 the train image in the second.  len_err: the row length's float_len_error / word_len_error.
+int match_single(const void* d_desc1, int n1, const void* d_desc2, int n2, int D, const char* len_err, int hamming,
+                 double ratio, int mutual, const double* d_kp1, const double* d_kp2, int kp_dim, int* d_match_q,
+                 int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim, int capacity, int* d_count,
+                 void* d_workspace, void* stream) {
+  if (!d_desc1 || !d_desc2 || !d_match_q || !d_match_t || !d_count || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
+  if (n1 < 1 || n2 < 2) return fail2(DGB200_E_ARG, "need n1 >= 1 query and n2 >= 2 train descriptors");
+  if (len_err) return fail2(DGB200_E_ARG, len_err);
+  if (d_x1y1 && (!d_kp1 || !d_kp2 || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  const int32_t qoff[3] = {0, n1, n1}, toff[3] = {0, 0, n2}, pair[2] = {0, 1};
+  std::vector<PairMeta> meta;
+  const int rc = build_meta(qoff, toff, 2, pair, 1, &meta);
+  if (rc) return rc;
+  return run_match(d_desc1, d_desc2, D, hamming, meta, ratio, mutual, d_kp1, d_kp2, kp_dim, d_match_q, d_match_t, d_x1y1,
+                   d_x2y2, out_dim, capacity, nullptr, d_count, d_workspace, (cudaStream_t)stream);
+}
+
+// Many pairs over one bank (dgb200_match_descriptors_batch_dev and its binary twin).
+int match_batch(const void* d_bank, const int32_t* img_offsets, int n_images, int D, const char* len_err, int hamming,
+                const int32_t* pairs, int n_pairs, double ratio, int mutual, const double* d_kp_bank, int kp_dim,
+                int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
+                int32_t* d_offsets_out, void* d_workspace, void* stream) {
+  if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
+  if (len_err) return fail2(DGB200_E_ARG, len_err);
+  if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  std::vector<PairMeta> meta;
+  const int rc = build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta);
+  if (rc) return rc;
+  if (!d_bank && meta[n_pairs].tile0 > 0) return fail2(DGB200_E_ARG, "null descriptor bank");
+  if (capacity < meta[n_pairs].row0) return fail2(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
+  return run_match(d_bank, d_bank, D, hamming, meta, ratio, mutual, d_kp_bank, d_kp_bank, kp_dim, d_match_q, d_match_t,
+                   d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream);
 }
 
 }  // namespace
@@ -578,17 +674,8 @@ int dgb200_match_descriptors_dev(const float* d_desc1, int n1, const float* d_de
                                  const double* d_kp1, const double* d_kp2, int kp_dim, int* d_match_q, int* d_match_t,
                                  double* d_x1y1, double* d_x2y2, int out_dim, int capacity, int* d_count, void* d_workspace,
                                  void* stream) {
-  if (!d_desc1 || !d_desc2 || !d_match_q || !d_match_t || !d_count || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
-  if (n1 < 1 || n2 < 2) return fail2(DGB200_E_ARG, "need n1 >= 1 query and n2 >= 2 train descriptors");
-  if (D < 4 || D > 256 || (D & 3)) return fail2(DGB200_E_ARG, "descriptor length must be a multiple of 4 in [4, 256]");
-  if (d_x1y1 && (!d_kp1 || !d_kp2 || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
-  // a batch of one pair: image 0 is the query image in the first bank, image 1 the train image in the second
-  const int32_t qoff[3] = {0, n1, n1}, toff[3] = {0, 0, n2}, pair[2] = {0, 1};
-  std::vector<PairMeta> meta;
-  const int rc = build_meta(qoff, toff, 2, pair, 1, &meta);
-  if (rc) return rc;
-  return run_match(d_desc1, d_desc2, D, meta, ratio, mutual, d_kp1, d_kp2, kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2,
-                   out_dim, capacity, nullptr, d_count, d_workspace, (cudaStream_t)stream);
+  return match_single(d_desc1, n1, d_desc2, n2, D, float_len_error(D), 0, ratio, mutual, d_kp1, d_kp2, kp_dim, d_match_q,
+                      d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_count, d_workspace, stream);
 }
 
 int dgb200_match_descriptors_batch_dev(const float* d_bank, const int32_t* img_offsets, int n_images, int D,
@@ -596,16 +683,26 @@ int dgb200_match_descriptors_batch_dev(const float* d_bank, const int32_t* img_o
                                        int kp_dim, int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
                                        int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
                                        void* stream) {
-  if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
-  if (D < 4 || D > 256 || (D & 3)) return fail2(DGB200_E_ARG, "descriptor length must be a multiple of 4 in [4, 256]");
-  if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
-  std::vector<PairMeta> meta;
-  const int rc = build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta);
-  if (rc) return rc;
-  if (!d_bank && meta[n_pairs].tile0 > 0) return fail2(DGB200_E_ARG, "null descriptor bank");
-  if (capacity < meta[n_pairs].row0) return fail2(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
-  return run_match(d_bank, d_bank, D, meta, ratio, mutual, d_kp_bank, d_kp_bank, kp_dim, d_match_q, d_match_t, d_x1y1,
-                   d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream);
+  return match_batch(d_bank, img_offsets, n_images, D, float_len_error(D), 0, pairs, n_pairs, ratio, mutual, d_kp_bank,
+                     kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, d_workspace, stream);
+}
+
+int dgb200_match_binary_descriptors_dev(const uint32_t* d_desc1, int n1, const uint32_t* d_desc2, int n2, int n_words,
+                                        double ratio, int mutual, const double* d_kp1, const double* d_kp2, int kp_dim,
+                                        int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim,
+                                        int capacity, int* d_count, void* d_workspace, void* stream) {
+  return match_single(d_desc1, n1, d_desc2, n2, n_words, word_len_error(n_words), 1, ratio, mutual, d_kp1, d_kp2, kp_dim,
+                      d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_count, d_workspace, stream);
+}
+
+int dgb200_match_binary_descriptors_batch_dev(const uint32_t* d_bank, const int32_t* img_offsets, int n_images,
+                                              int n_words, const int32_t* pairs, int n_pairs, double ratio, int mutual,
+                                              const double* d_kp_bank, int kp_dim, int* d_match_q, int* d_match_t,
+                                              double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
+                                              int32_t* d_offsets_out, void* d_workspace, void* stream) {
+  return match_batch(d_bank, img_offsets, n_images, n_words, word_len_error(n_words), 1, pairs, n_pairs, ratio, mutual,
+                     d_kp_bank, kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out,
+                     d_workspace, stream);
 }
 
 int dgb200_pose_from_fundamental_batch_dev(const double* d_F, const double* d_K1, const double* d_K2, int k_per_pair,

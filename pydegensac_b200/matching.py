@@ -8,6 +8,10 @@ descriptors go in, models and masks come out, nothing visits the host in between
     idx1, idx2, pts1, pts2 = match_descriptors(desc1, desc2, kp1, kp2, ratio=0.9)
     F, mask = pydegensac_b200.findFundamentalMatrixBatch(pts1[None], pts2[None], 0.5, 0.999, 50000)
 
+Binary descriptors (ORB, AKAZE, BRISK, FREAK: uint8 [n, B]) by Hamming distance, as cv2.NORM_HAMMING:
+
+    idx1, idx2, pts1, pts2 = match_descriptors(orb1, orb2, kp1, kp2, ratio=0.9, norm="hamming")
+
 Many image pairs at once (one matcher call, one RANSAC launch, no host read in between):
 
     m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
@@ -51,17 +55,55 @@ def batch_layout(counts, pairs):
     return BatchLayout(prefix(tiles), rows, prefix(n2), int(rows[-1]), int(n1.max()))
 
 
-def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False):
-    """Two-nearest-neighbour L2 matching + SNN ratio test (+ optional mutual nearest-neighbour check).
+def _check_norm(norm):
+    if norm not in ("l2", "hamming"):
+        raise ValueError("norm must be 'l2' or 'hamming', not %r" % (norm,))
+    return norm == "hamming"
 
-    desc1 [n1,D], desc2 [n2,D]: CUDA tensors (any float dtype; computed in float32), D a multiple of 4, <= 256.
+
+def _binary_words(descs):
+    """uint8 CUDA tensors [n_i, B] (one B in [1, 256]) -> one int32 tensor [sum n_i, W] of their rows, zero-padded to
+    W = ceil(B / 16) * 4 32-bit words (padding changes no Hamming distance; 16-byte rows keep the bulk copies)."""
+    import torch
+    dev = descs[0].device
+    if any(d.dtype != torch.uint8 for d in descs):
+        raise ValueError("norm='hamming' takes uint8 descriptor tensors [n, B] (the layout cv2 returns)")
+    if any(d.dim() != 2 for d in descs):
+        raise ValueError("expected binary descriptor tensors [n, B]")
+    B = int(descs[0].shape[1])
+    if any(int(d.shape[1]) != B for d in descs):
+        raise ValueError("binary descriptors of one call must all have the same length in bytes")
+    if not 1 <= B <= 256:
+        raise ValueError("binary descriptors must be 1 to 256 bytes long, not %d" % B)
+    if dev.type != "cuda" or any(d.device != dev for d in descs):
+        raise ValueError("expected CUDA descriptor tensors on one device")
+    W = (B + 15) // 16 * 4
+    rows = torch.zeros((sum(int(d.shape[0]) for d in descs), 4 * W), dtype=torch.uint8, device=dev)
+    rows[:, :B] = torch.cat(descs, 0)
+    return rows.view(torch.int32)
+
+
+def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False, norm="l2"):
+    """Two-nearest-neighbour matching + SNN ratio test (+ optional mutual nearest-neighbour check).
+
+    norm="l2": squared L2.  desc1 [n1,D], desc2 [n2,D]: CUDA tensors (any float dtype; computed in float32), D a
+    multiple of 4, <= 256; a query is accepted when d1 < ratio^2 * d2 (FP32, on the squared distances).
+    norm="hamming": binary descriptors (ORB 32 bytes, AKAZE 61, BRISK/FREAK 64) as uint8 CUDA tensors [n1,B], [n2,B]
+    with B in [1, 256]; the distance is the number of differing bits and a query is accepted when
+    float64(d1) < ratio * float64(d2) -- what cv2.BFMatcher(cv2.NORM_HAMMING).knnMatch(k=2) and the ratio test
+    `m.distance < ratio * n.distance` accept.
     kp1 [n1,>=2], kp2 [n2,>=2]: optional keypoint coordinate tensors (first two columns x, y; six columns carry the
     local affine shape through for the LAF check).
     Returns (idx1, idx2) int64 CUDA tensors of the accepted matches in ascending query order, plus (pts1, pts2) float64
     [N,2] (or [N,6]) CUDA tensors when keypoints were given."""
     import torch
-    d1 = desc1.to(torch.float32).contiguous()
-    d2 = desc2.to(torch.float32).contiguous()
+    hamming = _check_norm(norm)
+    if hamming:
+        words = _binary_words([desc1, desc2])     # one allocation; desc2's rows start 16-byte aligned
+        d1, d2 = words[:desc1.shape[0]], words[desc1.shape[0]:]
+    else:
+        d1 = desc1.to(torch.float32).contiguous()
+        d2 = desc2.to(torch.float32).contiguous()
     if d1.dim() != 2 or d2.dim() != 2 or d1.shape[1] != d2.shape[1] or not d1.is_cuda or d1.device != d2.device:
         raise ValueError("expected two CUDA descriptor tensors [n1,D], [n2,D] on the same device")
     n1, D = d1.shape
@@ -86,12 +128,13 @@ def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False)
             x2 = torch.empty((n1, out_dim), dtype=torch.float64, device=dev)
         stream = torch.cuda.current_stream(dev).cuda_stream
         vp = ctypes.c_void_p
-        rc = L.dgb200_match_descriptors_dev(vp(d1.data_ptr()), n1, vp(d2.data_ptr()), n2, D, ctypes.c_float(ratio),
-                                            int(bool(mutual)), vp(k1.data_ptr()) if k1 is not None else None,
-                                            vp(k2.data_ptr()) if k2 is not None else None, kp_dim, vp(mq.data_ptr()),
-                                            vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
-                                            vp(x2.data_ptr()) if x2 is not None else None, out_dim, n1,
-                                            vp(cnt.data_ptr()), vp(ws.data_ptr()), vp(stream))
+        fn, r = ((L.dgb200_match_binary_descriptors_dev, ctypes.c_double(ratio)) if hamming else
+                 (L.dgb200_match_descriptors_dev, ctypes.c_float(ratio)))
+        rc = fn(vp(d1.data_ptr()), n1, vp(d2.data_ptr()), n2, D, r, int(bool(mutual)),
+                vp(k1.data_ptr()) if k1 is not None else None, vp(k2.data_ptr()) if k2 is not None else None, kp_dim,
+                vp(mq.data_ptr()), vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
+                vp(x2.data_ptr()) if x2 is not None else None, out_dim, n1, vp(cnt.data_ptr()), vp(ws.data_ptr()),
+                vp(stream))
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
         n = int(cnt.item())          # the one host read of the front-end: how many tentatives there are
@@ -137,10 +180,11 @@ def pose_from_fundamental(F, K1, K2, pts1, pts2, mask=None):
     return R, t, good
 
 
-def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False):
+def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
     """match_descriptors over many image pairs in one call, output in the ragged layout of the offsets= entry points.
 
-    descs: list of I CUDA tensors [n_i, D] (n_i may be 0; converted to float32 like match_descriptors).
+    descs: list of I CUDA tensors [n_i, D] (n_i may be 0; converted to float32 like match_descriptors), or with
+    norm="hamming" uint8 tensors [n_i, B] with one B in [1, 256] (the distance and ratio test of match_descriptors).
     pairs: HOST [P,2] int array (numpy / list / CPU tensor) of (query image, train image); reading a CUDA tensor would
     synchronise, so one is refused.  kps: optional list of I tensors [n_i, k] (k >= 2; six columns carry the local
     affine shape through).
@@ -151,6 +195,7 @@ def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False):
     query image is empty or whose train image has fewer than 2 descriptors has no matches.  Asynchronous: nothing is
     read back from the device."""
     import torch
+    hamming = _check_norm(norm)
     if isinstance(pairs, torch.Tensor):
         if pairs.is_cuda:
             raise ValueError("pairs must be a host array: reading a CUDA tensor would synchronise")
@@ -158,11 +203,15 @@ def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False):
     if len(descs) < 1:
         raise ValueError("expected a non-empty list of descriptor tensors")
     dev = descs[0].device
-    ds = [d.to(torch.float32) for d in descs]
-    if not dev.type == "cuda" or any(d.dim() != 2 or d.device != dev or d.shape[1] != ds[0].shape[1] for d in ds):
-        raise ValueError("expected CUDA descriptor tensors [n_i, D] with one D, on one device")
+    if hamming:
+        ds = descs
+        bank = _binary_words(list(ds))
+    else:
+        ds = [d.to(torch.float32) for d in descs]
+        if not dev.type == "cuda" or any(d.dim() != 2 or d.device != dev or d.shape[1] != ds[0].shape[1] for d in ds):
+            raise ValueError("expected CUDA descriptor tensors [n_i, D] with one D, on one device")
+        bank = torch.cat(ds, 0).contiguous()
     counts = [int(d.shape[0]) for d in ds]
-    bank = torch.cat(ds, 0).contiguous()
     kbank = None
     if kps is not None:
         if len(kps) != len(ds):
@@ -172,12 +221,13 @@ def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False):
                 or ks[0].shape[1] < 2:
             raise ValueError("keypoint tensors must be [n_i, k] with one k >= 2")
         kbank = torch.cat(ks, 0).contiguous()
-    return _match_bank(bank, counts, pairs, kbank, ratio, mutual)
+    return _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming)
 
 
-def _match_bank(bank, counts, pairs, kbank, ratio, mutual):
+def _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming=False):
     """The batched matcher over a descriptor bank [R,D] (any 4-byte alignment) whose image i owns rows
-    sum(counts[:i]) .. sum(counts[:i+1])-1; kbank: keypoint rows of the same images or None."""
+    sum(counts[:i]) .. sum(counts[:i+1])-1: float32 rows, or with `hamming` binary rows of D 32-bit words (D a
+    multiple of 4); kbank: keypoint rows of the same images or None."""
     import torch
     pr = np.ascontiguousarray(np.asarray(pairs), dtype=np.int32)
     lay = batch_layout(counts, pr)
@@ -205,13 +255,13 @@ def _match_bank(bank, counts, pairs, kbank, ratio, mutual):
             x2 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
         stream = torch.cuda.current_stream(dev)
         vp = ctypes.c_void_p
-        rc = L.dgb200_match_descriptors_batch_dev(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D,
-                                                  pr.ctypes.data_as(i32), P, ctypes.c_float(ratio), int(bool(mutual)),
-                                                  vp(kbank.data_ptr()) if kbank is not None else None, kp_dim,
-                                                  vp(mq.data_ptr()), vp(mt.data_ptr()),
-                                                  vp(x1.data_ptr()) if x1 is not None else None,
-                                                  vp(x2.data_ptr()) if x2 is not None else None, out_dim, cap,
-                                                  vp(offsets.data_ptr()), vp(ws.data_ptr()), vp(stream.cuda_stream))
+        fn, r = ((L.dgb200_match_binary_descriptors_batch_dev, ctypes.c_double(ratio)) if hamming else
+                 (L.dgb200_match_descriptors_batch_dev, ctypes.c_float(ratio)))
+        rc = fn(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D, pr.ctypes.data_as(i32), P, r,
+                int(bool(mutual)), vp(kbank.data_ptr()) if kbank is not None else None, kp_dim, vp(mq.data_ptr()),
+                vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
+                vp(x2.data_ptr()) if x2 is not None else None, out_dim, cap, vp(offsets.data_ptr()), vp(ws.data_ptr()),
+                vp(stream.cuda_stream))
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return BatchMatches(mq.long(), mt.long(), x1, x2, offsets, lay.n_max)
