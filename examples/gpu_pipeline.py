@@ -3,6 +3,7 @@
 
     descriptors + keypoints (CUDA tensors)  ->  2-NN matching + SNN ratio test   (pydegensac_b200.matching, CUDA)
                                             ->  findHomography / findFundamentalMatrix (device-resident tensors)
+                                            ->  guided re-match inside F's epipolar band   (pydegensac_b200.matching, CUDA)
                                             ->  relative pose from F                      (pydegensac_b200.matching)
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
@@ -19,7 +20,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import match_descriptors, pose_from_fundamental
+from pydegensac_b200.matching import match_descriptors, match_descriptors_guided, pose_from_fundamental
 from pydegensac_b200.scenes import scene_F, _K
 
 
@@ -44,6 +45,9 @@ def main():
     print("tentative correspondences:", len(idx1))
     F, mask = pydegensac.findFundamentalMatrixBatch(pts1[None], pts2[None], 0.5, 0.999, 50000, seeds=[0])
     print("pydegensac_b200 found %d inliers" % int(mask.sum()))
+    # guided re-match: candidates of a query are the train keypoints within 1 px (Sampson) of its epipolar line
+    g = match_descriptors_guided([d1, d2], [[0, 1]], [kp1, kp2], F, 1.0, guide="F", ratio=0.9)
+    print("tentative correspondences: %d unguided, %d guided by F" % (len(idx1), int(g.offsets[1])))
     K = torch.from_numpy(_K).to(dev)
     R, t, good = pose_from_fundamental(F, K, K, pts1[None], pts2[None], mask)
     print("R =\n", R[0].cpu().numpy(), "\nt =", t[0].cpu().numpy(), " (%d correspondences in front of both cameras)" % int(good[0]))

@@ -203,6 +203,43 @@ int dgb200_match_binary_descriptors_batch_dev(const uint32_t* d_bank, const int3
                                               const double* d_kp_bank, int kp_dim, int* d_match_q, int* d_match_t,
                                               double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
                                               int32_t* d_offsets_out, void* d_workspace, void* stream);
+/* Guided matching: the batch matchers above with each pair's candidates restricted by a model of the pair, as after a
+ * first RANSAC pass (COLMAP's guided matching).  For pair p = (query image q, train image t), d_models + 9 p holds
+ * M_p (float64, row-major) and th = px_th * px_th (FP64).  With (xq, yq) = columns 0-1 of q's keypoint row i and
+ * (xt, yt) those of t's row j, train descriptor j is a CANDIDATE of query i when
+ *   guide = DGB200_GUIDE_F (x_t^T F x_q = 0, what dgb200_find_fundamental_* return): the engine's Sampson residual,
+ *     with rxc = (F0 xt + F3 yt) + F6, ryc = (F1 xt + F4 yt) + F7, rwc = (F2 xt + F5 yt) + F8,
+ *     rx = (F0 xq + F1 yq) + F2, ry = (F3 xq + F4 yq) + F5, r = (xq rxc + yq ryc) + rwc:
+ *     (r r) / (((rxc rxc + ryc ryc) + rx rx) + ry ry) <= th -- the rule that makes a correspondence an inlier of the
+ *     RANSAC mask at the same px_th;
+ *   guide = DGB200_GUIDE_H (x_t ~ H x_q, OpenCV convention, what dgb200_find_homography_* return):
+ *     w = (H6 xq + H7 yq) + H8, px = ((H0 xq + H1 yq) + H2) / w, py = ((H3 xq + H4 yq) + H5) / w,
+ *     dx = xt - px, dy = yt - py:  dx dx + dy dy <= th.
+ * Every operation is an IEEE double operation in the order written (no fused multiply-add).  A comparison that is not
+ * true fails, so an all-zero model (what the RANSAC returns when it finds none), a model with a NaN, or w = 0 with a
+ * finite px_th admits no candidate: such a pair gets ZERO matches.  Among its candidates each query keeps the two
+ * nearest train descriptors under the matcher's distance (squared L2 in FP32, or Hamming), ties to the lowest train
+ * index, d2 = +inf with fewer than two candidates; the ratio test and mutual check are the batch matcher's, so a query
+ * with exactly one candidate passes the ratio test for any ratio > 0, and with `mutual` a train's nearest query is taken
+ * over the queries whose gate admits it.  Output, ordering, the degenerate-pair rule, capacity, workspace
+ * (dgb200_match_batch_workspace_bytes) and errors are those of the batch matchers; in addition a null d_models, a null
+ * d_kp_bank or kp_dim < 2 (the gate needs the coordinates even when d_x1y1 is NULL), a guide other than the two below,
+ * or a negative or NaN px_th returns DGB200_E_ARG before any launch.  One pair is a batch of one pair over two images. */
+#define DGB200_GUIDE_F 0
+#define DGB200_GUIDE_H 1
+int dgb200_match_descriptors_guided_batch_dev(const float* d_bank, const int32_t* img_offsets, int n_images, int D,
+                                              const int32_t* pairs, int n_pairs, const double* d_models, int guide,
+                                              double px_th, float ratio, int mutual, const double* d_kp_bank, int kp_dim,
+                                              int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
+                                              int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                              void* stream);
+int dgb200_match_binary_descriptors_guided_batch_dev(const uint32_t* d_bank, const int32_t* img_offsets, int n_images,
+                                                     int n_words, const int32_t* pairs, int n_pairs,
+                                                     const double* d_models, int guide, double px_th, double ratio,
+                                                     int mutual, const double* d_kp_bank, int kp_dim, int* d_match_q,
+                                                     int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim,
+                                                     int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                                     void* stream);
 /* Pose from fundamental matrices: E = K2^T F K1, the four (R, t) candidates of its SVD, cheirality vote over the
  * correspondences with mask != 0 (NULL: all).  d_K1/d_K2: one 3x3 (k_per_pair = 0) or one per pair, row-major.
  * Outputs R [n_pairs][9] row-major, t [n_pairs][3] (unit length, x2 ~ R x1 + t), good [n_pairs] = supporters or NULL.

@@ -12,6 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIBPATH = os.path.join(_HERE, "libdegensac_b200.so")
 _lib = None
 FLAG_FINAL_LSQ = 1   # DGB200_FLAG_FINAL_LSQ
+GUIDE_F, GUIDE_H = 0, 1   # DGB200_GUIDE_F, DGB200_GUIDE_H
 
 
 class EngineUnavailable(RuntimeError):
@@ -58,7 +59,11 @@ def lib():
                                                           vp, vp]
         L.dgb200_match_binary_descriptors_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, cd, ci, vp, ci, vp, vp, vp, vp,
                                                                 ci, ci, vp, vp, vp]
-        L.dgb200_pose_from_fundamental_batch_dev.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
+        L.dgb200_match_descriptors_guided_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, vp, ci, cd, ctypes.c_float, ci,
+                                                                vp, ci, vp, vp, vp, vp, ci, ci, vp, vp, vp]
+        L.dgb200_match_binary_descriptors_guided_batch_dev.argtypes = [vp, i32, ci, ci, i32, ci, vp, ci, cd, cd, ci, vp,
+                                                                       ci, vp, vp, vp, vp, ci, ci, vp, vp, vp]
+        L.dgb200_pose_from_fundamental_batch_dev.argtypes =[vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p
         L.dgb200_last_error.restype = ctypes.c_char_p

@@ -88,7 +88,79 @@ struct MatchArgs {
   int mutual;                         // also track, per train descriptor, its nearest query (col_best)
   int* nn_idx; float* nn_d1; float* nn_d2;          // per query: nearest train index, distances of the two nearest
   unsigned long long* col_best;       // per train descriptor: (distance bits << 32 | query index), atomicMin
+  // guided matching only (a gate other than NoGate): per-pair models [n_pairs][9], keypoint rows of the banks'
+  // images [rows][kp_dim] (x, y in columns 0-1) and the squared pixel threshold
+  const double* models; const double* kq; const double* kt; int kp_dim; double th;
 };
+
+// ------------------------------------------------------------------------------------------------ guided matching
+// Gate policies of the matcher: which train descriptors of a pair count as candidates of a query.  A policy splits its
+// predicate into query terms (Q, registers of the query's thread), row terms (kTerms doubles per train row, computed
+// once per CTA and staged in shared memory beside the descriptors) and pass(), which combines them in exactly the
+// operation order of the unsplit expression (the library is compiled with -fmad=false), so that the gate is bit for bit
+// the expression written out in the header.  Every comparison is written so that NaN fails it.
+struct NoGate {             // plain matching: every train descriptor is a candidate
+  static constexpr bool kOn = false;
+  static constexpr int kTerms = 0;
+  struct Q {};
+};
+
+__device__ __forceinline__ double qnan() { return __longlong_as_double(0x7ff8000000000000ll); }
+
+// F (x_t^T F x_q = 0): the engine's Sampson residual dg::f_resid_sampson(F, xq, yq, xt, yt) <= th -- the rule that
+// makes a correspondence an inlier of the RANSAC mask.  f_res_terms: rxc, ryc, rwc depend on the train point only, rx,
+// ry on the query only; the denominator sums (((rxc^2 + ryc^2) + rx^2) + ry^2) left to right, so rxc^2 + ryc^2 is a
+// row term as well.
+struct EpipolarGate {
+  static constexpr bool kOn = true;
+  static constexpr int kTerms = 4;                     // rxc, ryc, rwc, rxc^2 + ryc^2
+  struct Q { double xq, yq, rx2, ry2; };
+  __device__ __forceinline__ static Q query(const double* F, double x, double y, bool valid) {
+    if (!valid) return Q{qnan(), qnan(), qnan(), qnan()};
+    const double rx = F[0] * x + F[1] * y + F[2];
+    const double ry = F[3] * x + F[4] * y + F[5];
+    return Q{x, y, rx * rx, ry * ry};
+  }
+  __device__ __forceinline__ static void row(const double* F, double x, double y, double* o) {
+    const double rxc = F[0] * x + F[3] * y + F[6];
+    const double ryc = F[1] * x + F[4] * y + F[7];
+    o[0] = rxc; o[1] = ryc; o[2] = F[2] * x + F[5] * y + F[8]; o[3] = rxc * rxc + ryc * ryc;
+  }
+  __device__ __forceinline__ static bool pass(const Q& q, const double* o, double th) {
+    const double r = q.xq * o[0] + q.yq * o[1] + o[2];
+    const double num = r * r;
+    const double den = o[3] + q.rx2 + q.ry2;
+    // Division-free pre-test on the same operands.  When t = th * den is a normal double it is at least
+    // th * den * (1 - 2^-53) (den > 0 then, since th >= 0), so num > 2 t means num / den > 2 (1 - 2^-53) th >= 1.5 th.
+    // The gap above any positive double is at most the double itself, so 1.5 th lies at or beyond the midpoint
+    // between th and its successor: the rounded quotient exceeds th and the exact test below would fail too.  2 t is
+    // exact or +inf (no rejection).  A zero, subnormal, infinite or NaN t, or a NaN num, goes to the exact test.
+    const double t = th * den;
+    if (t >= 2.2250738585072014e-308 && num > 2.0 * t) return false;
+    return num / den <= th;
+  }
+};
+
+// H (x_t ~ H x_q, row-major): the query's transfer (px, py) lies within px_th of the train point.  The transfer
+// depends on the query only; w = 0 or a NaN model gives a NaN or infinite distance, which fails.
+struct TransferGate {
+  static constexpr bool kOn = true;
+  static constexpr int kTerms = 2;                     // xt, yt
+  struct Q { double px, py; };
+  __device__ __forceinline__ static Q query(const double* H, double x, double y, bool valid) {
+    if (!valid) return Q{qnan(), qnan()};
+    const double w = H[6] * x + H[7] * y + H[8];
+    return Q{(H[0] * x + H[1] * y + H[2]) / w, (H[3] * x + H[4] * y + H[5]) / w};
+  }
+  __device__ __forceinline__ static void row(const double*, double x, double y, double* o) { o[0] = x; o[1] = y; }
+  __device__ __forceinline__ static bool pass(const Q& q, const double* o, double th) {
+    const double dx = o[0] - q.px, dy = o[1] - q.py;
+    return dx * dx + dy * dy <= th;
+  }
+};
+
+// The gate of one pair as nn2_tile sees it: the model, the query and train images' keypoint rows, th.
+struct GateCtx { const double* model; const double* kq; const double* kt; int kp_dim; double th; };
 
 // The distances of the matcher.  Each has a 4-byte element, reads rows 16 bytes at a time and accumulates four train
 // rows against one query row; key() maps a distance to 32 bits that order like it (the high word of col_best).
@@ -134,12 +206,12 @@ struct HammingDist {        // differing bits of binary rows of 32-bit words: on
 };
 
 // Two nearest train descriptors of the queries q0 .. q0+kTQ-1 of one pair under the distance Dist (ties go to the
-// lowest train index).  d1 [n1][D], d2 [n2][D] elements; nn_* and col_best are the pair's own segments.  Called by all
-// kMatchThreads threads of the CTA.
-template <class Dist>
+// lowest train index), among the candidates the gate admits (NoGate: all).  d1 [n1][D], d2 [n2][D] elements; nn_* and
+// col_best are the pair's own segments.  Called by all kMatchThreads threads of the CTA.
+template <class Dist, class Gate>
 __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, const typename Dist::Elem* d2, int n2,
                                          int D, int q0, int use_bulk, int mutual, int* nn_idx, float* nn_d1,
-                                         float* nn_d2, unsigned long long* col_best) {
+                                         float* nn_d2, unsigned long long* col_best, const GateCtx& gc) {
   using T = typename Dist::Elem;
   using Acc = typename Dist::Acc;
   extern __shared__ __align__(128) unsigned char msm[];
@@ -148,10 +220,16 @@ __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, 
   T* tq = reinterpret_cast<T*>(msm);                    // [kTQ][D + 4]
   T* tt = tq + kTQ * qs;                                // 2 stages x [kTT][D]
   const size_t stage_elems = (size_t)kTT * D;
+  // gated: 2 stages x [kTT][kTerms] row terms (double buffered with the descriptors), then the pair's model [9]
+  double* gt = reinterpret_cast<double*>(tt + 2 * stage_elems);
+  double* gm = gt + 2 * kTT * Gate::kTerms;
   const int tid = threadIdx.x, q = tid & 31, g = tid >> 5;
   for (int i = tid; i < kTQ * D; i += kMatchThreads) {
     const int r = i / D, c = i % D;
     tq[r * qs + c] = (q0 + r < n1) ? d1[(size_t)(q0 + r) * D + c] : T(0);
+  }
+  if constexpr (Gate::kOn) {
+    if (tid < 9) gm[tid] = gc.model[tid];
   }
   if (tid == 0) { mbar_init(&bar[0], 1); mbar_init(&bar[1], 1); }
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -170,10 +248,23 @@ __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, 
       const T* src = d2 + (size_t)t * kTT * D;
       for (int i = tid; i < rows * D; i += kMatchThreads) dst[i] = src[i];
     }
+    if constexpr (Gate::kOn) {       // the gate's row terms of the tile, one thread per train row
+      if (tid < rows) {
+        const double* kp = gc.kt + ((size_t)t * kTT + tid) * gc.kp_dim;
+        Gate::row(gm, kp[0], kp[1], gt + ((size_t)(t & 1) * kTT + tid) * Gate::kTerms);
+      }
+    }
   };
+  typename Gate::Q gq;
+  if constexpr (Gate::kOn) {
+    const bool valid = q0 + q < n1;
+    const double* kp = gc.kq + (size_t)(valid ? q0 + q : 0) * gc.kp_dim;
+    gq = Gate::query(gm, kp[0], kp[1], valid);      // a query past n1 gets NaN terms: no candidate
+  }
   float b1 = INFINITY, b2 = INFINITY;
   int i1 = -1;
   if (ntiles > 0) issue(0);
+  if constexpr (Gate::kOn) __syncthreads();           // tile 0's row terms (later tiles: the loop's barrier)
   for (int t = 0; t < ntiles; ++t) {
     if (t + 1 < ntiles) issue(t + 1);                 // next tile in flight behind this one's math
     if (use_bulk) mbar_wait(&bar[t & 1], (uint32_t)((t >> 1) & 1)); else __syncthreads();
@@ -182,6 +273,19 @@ __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, 
     const T* A = tq + q * qs;
     // this thread: train rows g*16 .. g*16+15 of the tile, four at a time (query chunk loaded once per four rows)
     for (int jb = g * 16; jb < g * 16 + 16 && jb < rows; jb += 4) {
+      bool ok[4] = {true, true, true, true};
+      if constexpr (Gate::kOn) {
+        // the gate of the four rows, then a warp vote: when it admits none of them for any of the warp's queries the
+        // warp skips their distances (warp-uniform branch)
+        const double* G = gt + ((size_t)(t & 1) * kTT + jb) * Gate::kTerms;
+        bool any = false;
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+          ok[u] = jb + u < rows && Gate::pass(gq, G + u * Gate::kTerms, gc.th);
+          any |= ok[u];
+        }
+        if (!__any_sync(0xffffffffu, any)) continue;
+      }
       Acc s0 = 0, s1 = 0, s2 = 0, s3 = 0;
       const T* B0 = B + (size_t)jb * D;
       const int r1 = (jb + 1 < rows) ? 1 : 0, r2 = (jb + 2 < rows) ? 2 : 0, r3 = (jb + 3 < rows) ? 3 : 0;
@@ -193,12 +297,15 @@ __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, 
         if (j < rows) {                                // (warp-uniform: g and rows are)
           const float s = (float)sv[u];
           const int gj = t * kTT + j;
-          if (s < b1 || (s == b1 && gj < i1)) { b2 = b1; b1 = s; i1 = gj; }
-          else if (s < b2) b2 = s;
+          if (ok[u]) {                                 // (NoGate: always) a rejected candidate updates nothing
+            if (s < b1 || (s == b1 && gj < i1)) { b2 = b1; b1 = s; i1 = gj; }
+            else if (s < b2) b2 = s;
+          }
           if (mutual) {
             // nearest QUERY of train descriptor gj among this warp's 32 queries, then one atomic per warp and row
-            unsigned long long key = (q0 + q < n1) ? (((unsigned long long)Dist::key(sv[u]) << 32) | (unsigned)(q0 + q))
-                                                    : 0xffffffffffffffffull;
+            unsigned long long key = (ok[u] && q0 + q < n1)
+                                         ? (((unsigned long long)Dist::key(sv[u]) << 32) | (unsigned)(q0 + q))
+                                         : 0xffffffffffffffffull;
 #pragma unroll
             for (int o = 16; o > 0; o >>= 1) {
               const unsigned long long other = __shfl_xor_sync(0xffffffffu, key, o);
@@ -233,7 +340,7 @@ __device__ __forceinline__ void nn2_tile(const typename Dist::Elem* d1, int n1, 
 
 // One flat grid over the (pair, kTQ-query tile) work items of the whole batch: CTA b finds its pair by binary search
 // over the tile prefix (the last pair whose first tile is <= b: pairs without tiles share their successor's prefix).
-template <class Dist>
+template <class Dist, class Gate>
 __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
   using T = typename Dist::Elem;
   const int b = blockIdx.x;
@@ -243,9 +350,20 @@ __global__ void __launch_bounds__(kMatchThreads) nn2_kernel(MatchArgs a) {
     if (a.meta[mid].tile0 <= b) lo = mid; else hi = mid - 1;
   }
   const PairMeta m = a.meta[lo];
-  nn2_tile<Dist>((const T*)(a.qbank + (size_t)m.qrow * a.D), m.n1, (const T*)(a.tbank + (size_t)m.trow * a.D), m.n2, a.D,
-                 (b - m.tile0) * kTQ, a.use_bulk, a.mutual, a.nn_idx + m.row0, a.nn_d1 + m.row0, a.nn_d2 + m.row0,
-                 a.col_best + m.col0);
+  GateCtx gc{};
+  if constexpr (Gate::kOn)
+    gc = GateCtx{a.models + (size_t)lo * 9, a.kq + (size_t)m.qrow * a.kp_dim, a.kt + (size_t)m.trow * a.kp_dim, a.kp_dim,
+                 a.th};
+  nn2_tile<Dist, Gate>((const T*)(a.qbank + (size_t)m.qrow * a.D), m.n1, (const T*)(a.tbank + (size_t)m.trow * a.D), m.n2,
+                       a.D, (b - m.tile0) * kTQ, a.use_bulk, a.mutual, a.nn_idx + m.row0, a.nn_d1 + m.row0,
+                       a.nn_d2 + m.row0, a.col_best + m.col0, gc);
+}
+
+// shared memory of nn2_kernel<Dist, Gate>: the query tile, two descriptor stages, and when gated two stages of row
+// terms and the model (every element type of the descriptors is 4 bytes)
+size_t nn2_smem_bytes(int D, int terms) {
+  return sizeof(float) * ((size_t)kTQ * (D + 4) + 2 * (size_t)kTT * D) +
+         (terms ? sizeof(double) * (2 * (size_t)kTT * terms + 9) : 0);
 }
 
 constexpr int kSelThreads = 512;
@@ -551,10 +669,14 @@ int build_meta(const int32_t* qoff, const int32_t* toff, int n_images, const int
 
 // The matcher over a checked batch, asynchronous on st: metadata upload, 2-NN over all work items, per-pair counts,
 // scan, ordered write.  The banks hold float rows of D floats (squared L2; ratio is a float's value) or, when
-// `hamming`, binary rows of D 32-bit words.  offsets == nullptr: a workspace segment holds them.
+// `hamming`, binary rows of D 32-bit words.  offsets == nullptr: a workspace segment holds them.  guide: kNoGuide, or
+// DGB200_GUIDE_F / DGB200_GUIDE_H with per-pair models [P][9] and the squared threshold th (the keypoint banks then
+// give the gate its coordinates).
+constexpr int kNoGuide = -1;
 int run_match(const void* qbank, const void* tbank, int D, int hamming, const std::vector<PairMeta>& meta, double ratio,
               int mutual, const double* kq, const double* kt, int kp_dim, int* match_q, int* match_t, double* x1y1,
-              double* x2y2, int out_dim, int cap, int* offsets, int* count_out, void* workspace, cudaStream_t st) {
+              double* x2y2, int out_dim, int cap, int* offsets, int* count_out, void* workspace, cudaStream_t st,
+              int guide = kNoGuide, const double* models = nullptr, double th = 0.0) {
   const int P = (int)meta.size() - 1;
   const PairMeta& tot = meta[P];
   auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -571,13 +693,23 @@ int run_match(const void* qbank, const void* tbank, int D, int hamming, const st
   a.qbank = (const float*)qbank; a.tbank = (const float*)tbank; a.meta = d_meta; a.n_pairs = P; a.D = D;
   a.use_bulk = (((uintptr_t)tbank) & 15) == 0 ? 1 : 0;   // every image's rows then are too (D % 4 == 0)
   a.mutual = mutual;
+  a.models = models; a.kq = kq; a.kt = kt; a.kp_dim = kp_dim; a.th = th;
   // pageable source: the runtime stages it before returning, the copy itself is ordered on st like the kernels
   CU2(cudaMemcpyAsync(d_meta, meta.data(), sizeof(PairMeta) * meta.size(), cudaMemcpyHostToDevice, st));
   if (tot.tile0 > 0) {
     if (mutual) CU2(cudaMemsetAsync(a.col_best, 0xff, sizeof(unsigned long long) * (size_t)tot.col0, st));
-    // (both element types are 4 bytes)
-    const size_t smem = sizeof(float) * ((size_t)kTQ * (D + 4) + 2 * (size_t)kTT * D);
-    void (*kern)(MatchArgs) = hamming ? nn2_kernel<HammingDist> : nn2_kernel<L2Dist>;
+    void (*kern)(MatchArgs);
+    size_t smem;
+    if (guide == DGB200_GUIDE_F) {
+      kern = hamming ? nn2_kernel<HammingDist, EpipolarGate> : nn2_kernel<L2Dist, EpipolarGate>;
+      smem = nn2_smem_bytes(D, EpipolarGate::kTerms);
+    } else if (guide == DGB200_GUIDE_H) {
+      kern = hamming ? nn2_kernel<HammingDist, TransferGate> : nn2_kernel<L2Dist, TransferGate>;
+      smem = nn2_smem_bytes(D, TransferGate::kTerms);
+    } else {
+      kern = hamming ? nn2_kernel<HammingDist, NoGate> : nn2_kernel<L2Dist, NoGate>;
+      smem = nn2_smem_bytes(D, 0);
+    }
     CU2(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<tot.tile0, kMatchThreads, smem, st>>>(a);
     CU2(cudaGetLastError());
@@ -625,21 +757,29 @@ int match_single(const void* d_desc1, int n1, const void* d_desc2, int n2, int D
                    d_x2y2, out_dim, capacity, nullptr, d_count, d_workspace, (cudaStream_t)stream);
 }
 
-// Many pairs over one bank (dgb200_match_descriptors_batch_dev and its binary twin).
+// Many pairs over one bank (dgb200_match_descriptors_batch_dev and its binary twin; with a guide, the guided twins).
 int match_batch(const void* d_bank, const int32_t* img_offsets, int n_images, int D, const char* len_err, int hamming,
                 const int32_t* pairs, int n_pairs, double ratio, int mutual, const double* d_kp_bank, int kp_dim,
                 int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
-                int32_t* d_offsets_out, void* d_workspace, void* stream) {
+                int32_t* d_offsets_out, void* d_workspace, void* stream, bool guided = false, int guide = kNoGuide,
+                const double* d_models = nullptr, double px_th = 0.0) {
   if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
   if (len_err) return fail2(DGB200_E_ARG, len_err);
   if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  if (guided) {
+    if (!d_models) return fail2(DGB200_E_ARG, "null model array");
+    if (!d_kp_bank || kp_dim < 2) return fail2(DGB200_E_ARG, "guided matching needs the keypoint bank (kp_dim >= 2)");
+    if (guide != DGB200_GUIDE_F && guide != DGB200_GUIDE_H) return fail2(DGB200_E_ARG, "guide must be DGB200_GUIDE_F or DGB200_GUIDE_H");
+    if (!(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+  }
   std::vector<PairMeta> meta;
   const int rc = build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta);
   if (rc) return rc;
   if (!d_bank && meta[n_pairs].tile0 > 0) return fail2(DGB200_E_ARG, "null descriptor bank");
   if (capacity < meta[n_pairs].row0) return fail2(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
   return run_match(d_bank, d_bank, D, hamming, meta, ratio, mutual, d_kp_bank, d_kp_bank, kp_dim, d_match_q, d_match_t,
-                   d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream);
+                   d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream,
+                   guided ? guide : kNoGuide, d_models, px_th * px_th);
 }
 
 }  // namespace
@@ -705,7 +845,30 @@ int dgb200_match_binary_descriptors_batch_dev(const uint32_t* d_bank, const int3
                      d_workspace, stream);
 }
 
-int dgb200_pose_from_fundamental_batch_dev(const double* d_F, const double* d_K1, const double* d_K2, int k_per_pair,
+int dgb200_match_descriptors_guided_batch_dev(const float* d_bank, const int32_t* img_offsets, int n_images, int D,
+                                              const int32_t* pairs, int n_pairs, const double* d_models, int guide,
+                                              double px_th, float ratio, int mutual, const double* d_kp_bank, int kp_dim,
+                                              int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2,
+                                              int out_dim, int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                              void* stream) {
+  return match_batch(d_bank, img_offsets, n_images, D, float_len_error(D), 0, pairs, n_pairs, ratio, mutual, d_kp_bank,
+                     kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, d_workspace, stream,
+                     true, guide, d_models, px_th);
+}
+
+int dgb200_match_binary_descriptors_guided_batch_dev(const uint32_t* d_bank, const int32_t* img_offsets, int n_images,
+                                                     int n_words, const int32_t* pairs, int n_pairs,
+                                                     const double* d_models, int guide, double px_th, double ratio,
+                                                     int mutual, const double* d_kp_bank, int kp_dim, int* d_match_q,
+                                                     int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim,
+                                                     int capacity, int32_t* d_offsets_out, void* d_workspace,
+                                                     void* stream) {
+  return match_batch(d_bank, img_offsets, n_images, n_words, word_len_error(n_words), 1, pairs, n_pairs, ratio, mutual,
+                     d_kp_bank, kp_dim, d_match_q, d_match_t, d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out,
+                     d_workspace, stream, true, guide, d_models, px_th);
+}
+
+int dgb200_pose_from_fundamental_batch_dev(const double* d_F,const double* d_K1, const double* d_K2, int k_per_pair,
                                            const double* d_x1y1, const double* d_x2y2, const uint8_t* d_mask, int n_pairs,
                                            int n, int dim, double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                            void* stream) {

@@ -17,6 +17,10 @@ Many image pairs at once (one matcher call, one RANSAC launch, no host read in b
     m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
     F, mask = pydegensac_b200.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, offsets=m.offsets,
                                                          n_max=m.n_max)
+
+Guided re-match with the models found (candidates: the train keypoints within px_th of the epipolar line / transfer):
+
+    g = match_descriptors_guided(descs, pairs, kps, F, 1.0, guide="F")
 """
 import collections
 import ctypes
@@ -194,12 +198,65 @@ def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, nor
     match count.  capacity is the sum of the query images' counts; rows past offsets[P] are unspecified.  A pair whose
     query image is empty or whose train image has fewer than 2 descriptors has no matches.  Asynchronous: nothing is
     read back from the device."""
-    import torch
     hamming = _check_norm(norm)
+    pairs = _host_pairs(pairs)
+    bank, counts, kbank = _banks(descs, kps, hamming)
+    return _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming)
+
+
+def match_descriptors_guided(descs, pairs, kps, models, px_th, guide="F", ratio=0.9, mutual=False, norm="l2"):
+    """Guided matching: match_descriptors_batch with each pair's candidates restricted by a model of the pair.
+
+    After a first pass (match_descriptors_batch, then findFundamentalMatrixBatch / findHomographyBatch on its ragged
+    output), match the descriptors again, counting as candidates of a query only the train keypoints the pair's model
+    allows: guide="F" (x_t^T F x_q = 0): the engine's Sampson residual of (query, train) at most px_th^2 -- the
+    RANSAC's own inlier rule; guide="H" (x_t ~ H x_q): the query's transfer H x_q within px_th pixels of the train
+    keypoint.  The 2-NN, ratio test and mutual check then run among those candidates; a query with one candidate passes
+    the ratio test.  Repeated texture defeats the plain ratio test (the second neighbour is a look-alike elsewhere in the
+    image); inside the gate the look-alike is usually gone, so many true matches come back.
+
+    descs, pairs, ratio, mutual, norm: as match_descriptors_batch.  kps: list of I keypoint tensors [n_i, k] (k >= 2,
+    x and y in the first two columns), required.  models: [P,3,3] or [P,9] float64, row-major, in the pair order of
+    `pairs` (what findFundamentalMatrixBatch / findHomographyBatch return); a float64 CUDA tensor on the descriptors'
+    device is used in place, other input is uploaded.  A pair whose model is all zeros (no model found) or holds a NaN
+    gets no matches.  Returns BatchMatches like match_descriptors_batch; nothing is read back from the device."""
+    import torch
+    if guide not in ("F", "H"):
+        raise ValueError("guide must be 'F' or 'H', not %r" % (guide,))
+    px_th = float(px_th)
+    if not px_th >= 0.0:
+        raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
+    hamming = _check_norm(norm)
+    pairs = _host_pairs(pairs)
+    if kps is None:
+        raise ValueError("guided matching needs the keypoints of every image (kps)")
+    P = len(np.asarray(pairs))
+    if not isinstance(models, torch.Tensor):
+        models = np.array(models, dtype=np.float64)      # (a copy: torch wants a writable array)
+    if tuple(models.shape) not in ((P, 9), (P, 3, 3)):
+        raise ValueError("models must be [P,3,3] or [P,9] with P = %d pairs, not %s" % (P, list(models.shape)))
+    bank, counts, kbank = _banks(descs, kps, hamming)
+    dev = bank.device
+    if isinstance(models, torch.Tensor) and models.is_cuda and models.device != dev:
+        raise ValueError("models must be on the descriptors' device")
+    M = torch.as_tensor(models).to(device=dev, dtype=torch.float64).contiguous().view(P, 9)
+    return _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming,
+                       guide=(_cabi.GUIDE_F if guide == "F" else _cabi.GUIDE_H), models=M, px_th=px_th)
+
+
+def _host_pairs(pairs):
+    import torch
     if isinstance(pairs, torch.Tensor):
         if pairs.is_cuda:
             raise ValueError("pairs must be a host array: reading a CUDA tensor would synchronise")
         pairs = pairs.numpy()
+    return pairs
+
+
+def _banks(descs, kps, hamming):
+    """descriptor bank [R,D] (float32, or binary words), per-image counts and keypoint bank [R,k] float64 (or None)
+    of the lists taken by match_descriptors_batch"""
+    import torch
     if len(descs) < 1:
         raise ValueError("expected a non-empty list of descriptor tensors")
     dev = descs[0].device
@@ -221,13 +278,14 @@ def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, nor
                 or ks[0].shape[1] < 2:
             raise ValueError("keypoint tensors must be [n_i, k] with one k >= 2")
         kbank = torch.cat(ks, 0).contiguous()
-    return _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming)
+    return bank, counts, kbank
 
 
-def _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming=False):
+def _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming=False, guide=None, models=None, px_th=0.0):
     """The batched matcher over a descriptor bank [R,D] (any 4-byte alignment) whose image i owns rows
     sum(counts[:i]) .. sum(counts[:i+1])-1: float32 rows, or with `hamming` binary rows of D 32-bit words (D a
-    multiple of 4); kbank: keypoint rows of the same images or None."""
+    multiple of 4); kbank: keypoint rows of the same images or None.  guide (_cabi.GUIDE_F / GUIDE_H): guided matching
+    with models, a float64 CUDA tensor [P,9], and px_th."""
     import torch
     pr = np.ascontiguousarray(np.asarray(pairs), dtype=np.int32)
     lay = batch_layout(counts, pr)
@@ -255,9 +313,15 @@ def _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming=False):
             x2 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
         stream = torch.cuda.current_stream(dev)
         vp = ctypes.c_void_p
-        fn, r = ((L.dgb200_match_binary_descriptors_batch_dev, ctypes.c_double(ratio)) if hamming else
-                 (L.dgb200_match_descriptors_batch_dev, ctypes.c_float(ratio)))
-        rc = fn(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D, pr.ctypes.data_as(i32), P, r,
+        r = ctypes.c_double(ratio) if hamming else ctypes.c_float(ratio)
+        guided = ()
+        if guide is None:
+            fn = L.dgb200_match_binary_descriptors_batch_dev if hamming else L.dgb200_match_descriptors_batch_dev
+        else:
+            fn = (L.dgb200_match_binary_descriptors_guided_batch_dev if hamming else
+                  L.dgb200_match_descriptors_guided_batch_dev)
+            guided = (vp(models.data_ptr()), int(guide), ctypes.c_double(px_th))
+        rc = fn(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D, pr.ctypes.data_as(i32), P, *guided, r,
                 int(bool(mutual)), vp(kbank.data_ptr()) if kbank is not None else None, kp_dim, vp(mq.data_ptr()),
                 vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
                 vp(x2.data_ptr()) if x2 is not None else None, out_dim, cap, vp(offsets.data_ptr()), vp(ws.data_ptr()),
