@@ -248,6 +248,28 @@ int dgb200_pose_from_fundamental_batch_dev(const double* d_F, const double* d_K1
                                            const double* d_x1y1, const double* d_x2y2, const uint8_t* d_mask, int n_pairs,
                                            int n, int dim, double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                            void* stream);
+/* Pose from F over a RAGGED batch, as dgb200_find_fundamental_ragged_dev leaves it: pair p owns rows
+ * d_offsets[p] .. d_offsets[p+1]-1 (DEVICE int32 [n_pairs+1], read on the device only) of d_x1y1 / d_x2y2
+ * [rows][dim] float64 and d_mask [rows] (NULL: every row).  d_F [n_pairs][9] row-major (x2^T F x1 = 0), K as above.
+ * Per pair, the candidates, the vote and the tie rule of the dense entry point, so R, t, good equal a dense call on
+ * the pair alone.  Per row r, with x1 = K1^-1 [p1; 1], x2 = K2^-1 [p2; 1] and (l1, l2) the least-squares depths of
+ * l1 R x1 + t = l2 x2 under the chosen (R, t):
+ *   d_points_out [rows][3]  midpoint 0.5 (l1 x1 + R^T (l2 x2 - t)): camera 1's frame, units of the baseline (|t| = 1);
+ *   d_in_front_out [rows]   mask[r] && l1 > 0 && l2 > 0 (so good[p] is the pair's sum of it);
+ *   d_angle_out [rows]      parallax angle atan2(|x1 x R^T x2|, x1 . R^T x2) in radians, in [0, pi].
+ * d_median_angle_out [n_pairs]: the median of the angles of the pair's in-front rows (the mean of the two middle values
+ * for an even count, as np.median), exact for any pair length; NaN when no row is in front.  A pair whose F is all zero
+ * (no model) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, in_front = 0 and a NaN median.  Offsets
+ * that decrease, are negative or pass `rows` make an empty pair: no row is read or written.  d_mask and d_good_out may
+ * be NULL; the row arrays may be NULL when rows = 0; every other buffer is required.  A null required buffer,
+ * n_pairs < 1, rows < 0 or dim < 2 returns DGB200_E_ARG before any launch.  Asynchronous on `stream`, one kernel, no
+ * workspace. */
+int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K1, const double* d_K2, int k_per_pair,
+                                            const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets,
+                                            int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                            double* d_R_out, double* d_t_out, int32_t* d_good_out,
+                                            double* d_points_out, uint8_t* d_in_front_out, double* d_angle_out,
+                                            double* d_median_angle_out, void* stream);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

@@ -499,10 +499,70 @@ __device__ inline double det3r(const double* A) {
   return A[0] * (A[4] * A[8] - A[5] * A[7]) - A[1] * (A[3] * A[8] - A[5] * A[6]) + A[2] * (A[3] * A[7] - A[4] * A[6]);
 }
 
-// One warp per pair.  Lane 0 factors E (one-sided Jacobi SVD, la.h) and builds the four candidates; all lanes vote:
-// a correspondence supports (R, t) when its two-view triangulation lambda1 R x1 + t = lambda2 x2 (least squares in
-// lambda) has both depths positive.  Result: the candidate with the most supporters (first in the order
-// (R1,+t), (R1,-t), (R2,+t), (R2,-t) on ties), t of unit length.
+// The pieces of pose from F that the dense and the ragged kernel share, so that both give the same bits.
+// E = K2^T F K1, factored by the one-sided Jacobi SVD (la.h), and its four (R, t) candidates into cand[4][12] =
+// (R row-major [9], t [3]) in the order (R1,+t), (R1,-t), (R2,+t), (R2,-t); t = the third column of U, unit length.
+__device__ __forceinline__ void pose_candidates(const double* F, const double* K1, const double* K2, double* cand) {
+  double K2t[9], tmp[9], E[9];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) K2t[3 * i + j] = K2[3 * j + i];
+  mat3_mul(K2t, F, tmp);
+  mat3_mul(tmp, K1, E);
+  // E = U S V^T with G = E V (orthogonal columns, norms = singular values)
+  double G[9], V[9], sv[3];
+  dg::svd3_onesided(E, G, V, sv);
+  int o[3] = {0, 1, 2};                   // sort singular values, largest first
+  for (int i = 0; i < 3; ++i) for (int j = i + 1; j < 3; ++j) if (sv[o[j]] > sv[o[i]]) { const int tt = o[i]; o[i] = o[j]; o[j] = tt; }
+  double U[9], Vs[9];
+  for (int c = 0; c < 2; ++c) {
+    const int k = o[c];
+    const double inv = sv[k] > 0 ? 1.0 / sv[k] : 0.0;
+    for (int r = 0; r < 3; ++r) { U[3 * r + c] = G[3 * r + k] * inv; Vs[3 * r + c] = V[3 * r + k]; }
+  }
+  {  // third columns: cross products (unit, orthogonal), so that det(U) = det(V) = +1
+    const double u0[3] = {U[0], U[3], U[6]}, u1[3] = {U[1], U[4], U[7]}, v0[3] = {Vs[0], Vs[3], Vs[6]}, v1[3] = {Vs[1], Vs[4], Vs[7]};
+    double cu[3], cv[3];
+    dg::cross3(cu, u0, u1); dg::cross3(cv, v0, v1);
+    for (int r = 0; r < 3; ++r) { U[3 * r + 2] = cu[r]; Vs[3 * r + 2] = cv[r]; }
+  }
+  const double W[9] = {0, -1, 0, 1, 0, 0, 0, 0, 1}, Wt[9] = {0, 1, 0, -1, 0, 0, 0, 0, 1};
+  double Vt[9], UW[9], R1[9], R2[9];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Vt[3 * i + j] = Vs[3 * j + i];
+  mat3_mul(U, W, UW); mat3_mul(UW, Vt, R1);
+  mat3_mul(U, Wt, UW); mat3_mul(UW, Vt, R2);
+  for (int c = 0; c < 4; ++c) {
+    const double* Rc = (c < 2) ? R1 : R2;
+    const double sgn = (c & 1) ? -1.0 : 1.0;
+    for (int i = 0; i < 9; ++i) cand[12 * c + i] = Rc[i];
+    for (int r = 0; r < 3; ++r) cand[12 * c + 9 + r] = sgn * U[3 * r + 2];
+  }
+}
+
+// Normalised ray x = ki [px; py; 1] of a pixel.
+__device__ __forceinline__ void pose_ray(const double* ki, double px, double py, double* x) {
+  x[0] = ki[0] * px + ki[1] * py + ki[2];
+  x[1] = ki[3] * px + ki[4] * py + ki[5];
+  x[2] = ki[6] * px + ki[7] * py + ki[8];
+}
+
+// Two-view triangulation under (R, t): the least-squares depths (l1, l2) of l1 R x1 + t = l2 x2.
+__device__ __forceinline__ void pose_depths(const double* Rc, const double* tc, const double* x1, const double* x2,
+                                            double* l1, double* l2) {
+  const double a1[3] = {Rc[0] * x1[0] + Rc[1] * x1[1] + Rc[2] * x1[2], Rc[3] * x1[0] + Rc[4] * x1[1] + Rc[5] * x1[2],
+                        Rc[6] * x1[0] + Rc[7] * x1[1] + Rc[8] * x1[2]};
+  // minimise | l1 a1 - l2 x2 + t |: normal equations of the 3 x 2 system [a1, -x2] (l1, l2)^T = -t
+  const double aa = a1[0] * a1[0] + a1[1] * a1[1] + a1[2] * a1[2];
+  const double bb = x2[0] * x2[0] + x2[1] * x2[1] + x2[2] * x2[2];
+  const double ab = a1[0] * x2[0] + a1[1] * x2[1] + a1[2] * x2[2];
+  const double at = a1[0] * tc[0] + a1[1] * tc[1] + a1[2] * tc[2];
+  const double bt = x2[0] * tc[0] + x2[1] * tc[1] + x2[2] * tc[2];
+  const double det = aa * bb - ab * ab;
+  *l1 = (-at * bb + ab * bt) / det;
+  *l2 = (aa * bt - ab * at) / det;
+}
+
+// One warp per pair.  Lane 0 factors E and builds the four candidates; all lanes vote: a correspondence supports
+// (R, t) when its two-view triangulation (pose_depths) has both depths positive.  Result: the candidate with the most
+// supporters (first in the order (R1,+t), (R1,-t), (R2,+t), (R2,-t) on ties), t of unit length.
 __global__ void pose_kernel(PoseArgs a) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (warp >= a.n_pairs) return;
@@ -521,41 +581,7 @@ __global__ void pose_kernel(PoseArgs a) {
     dg::inv3(m);
     for (int i = 0; i < 9; ++i) k2i[i] = m[i];
   }
-  if (lane == 0) {
-    const double* F = a.F + (size_t)p * 9;
-    double K2t[9], tmp[9], E[9];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) K2t[3 * i + j] = K2[3 * j + i];
-    mat3_mul(K2t, F, tmp);
-    mat3_mul(tmp, K1, E);
-    // E = U S V^T with G = E V (orthogonal columns, norms = singular values)
-    double G[9], V[9], sv[3];
-    dg::svd3_onesided(E, G, V, sv);
-    int o[3] = {0, 1, 2};                   // sort singular values, largest first
-    for (int i = 0; i < 3; ++i) for (int j = i + 1; j < 3; ++j) if (sv[o[j]] > sv[o[i]]) { const int tt = o[i]; o[i] = o[j]; o[j] = tt; }
-    double U[9], Vs[9];
-    for (int c = 0; c < 2; ++c) {
-      const int k = o[c];
-      const double inv = sv[k] > 0 ? 1.0 / sv[k] : 0.0;
-      for (int r = 0; r < 3; ++r) { U[3 * r + c] = G[3 * r + k] * inv; Vs[3 * r + c] = V[3 * r + k]; }
-    }
-    {  // third columns: cross products (unit, orthogonal), so that det(U) = det(V) = +1
-      const double u0[3] = {U[0], U[3], U[6]}, u1[3] = {U[1], U[4], U[7]}, v0[3] = {Vs[0], Vs[3], Vs[6]}, v1[3] = {Vs[1], Vs[4], Vs[7]};
-      double cu[3], cv[3];
-      dg::cross3(cu, u0, u1); dg::cross3(cv, v0, v1);
-      for (int r = 0; r < 3; ++r) { U[3 * r + 2] = cu[r]; Vs[3 * r + 2] = cv[r]; }
-    }
-    const double W[9] = {0, -1, 0, 1, 0, 0, 0, 0, 1}, Wt[9] = {0, 1, 0, -1, 0, 0, 0, 0, 1};
-    double Vt[9], UW[9], R1[9], R2[9];
-    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) Vt[3 * i + j] = Vs[3 * j + i];
-    mat3_mul(U, W, UW); mat3_mul(UW, Vt, R1);
-    mat3_mul(U, Wt, UW); mat3_mul(UW, Vt, R2);
-    for (int c = 0; c < 4; ++c) {
-      const double* Rc = (c < 2) ? R1 : R2;
-      const double sgn = (c & 1) ? -1.0 : 1.0;
-      for (int i = 0; i < 9; ++i) cand[12 * c + i] = Rc[i];
-      for (int r = 0; r < 3; ++r) cand[12 * c + 9 + r] = sgn * U[3 * r + 2];
-    }
-  }
+  if (lane == 0) pose_candidates(a.F + (size_t)p * 9, K1, K2, cand);
   __syncwarp();
   int votes[4] = {0, 0, 0, 0};
   const double* g1 = a.x1y1 + (size_t)p * a.n * a.dim;
@@ -563,23 +589,12 @@ __global__ void pose_kernel(PoseArgs a) {
   const unsigned char* mk = a.mask ? a.mask + (size_t)p * a.n : nullptr;
   for (int i = lane; i < a.n; i += 32) {
     if (mk && !mk[i]) continue;
-    const double px1 = g1[(size_t)i * a.dim], py1 = g1[(size_t)i * a.dim + 1], px2 = g2[(size_t)i * a.dim], py2 = g2[(size_t)i * a.dim + 1];
-    const double x1[3] = {k1i[0] * px1 + k1i[1] * py1 + k1i[2], k1i[3] * px1 + k1i[4] * py1 + k1i[5], k1i[6] * px1 + k1i[7] * py1 + k1i[8]};
-    const double x2[3] = {k2i[0] * px2 + k2i[1] * py2 + k2i[2], k2i[3] * px2 + k2i[4] * py2 + k2i[5], k2i[6] * px2 + k2i[7] * py2 + k2i[8]};
+    double x1[3], x2[3];
+    pose_ray(k1i, g1[(size_t)i * a.dim], g1[(size_t)i * a.dim + 1], x1);
+    pose_ray(k2i, g2[(size_t)i * a.dim], g2[(size_t)i * a.dim + 1], x2);
     for (int c = 0; c < 4; ++c) {
-      const double* Rc = cand + 12 * c;
-      const double* tc = Rc + 9;
-      const double a1[3] = {Rc[0] * x1[0] + Rc[1] * x1[1] + Rc[2] * x1[2], Rc[3] * x1[0] + Rc[4] * x1[1] + Rc[5] * x1[2],
-                            Rc[6] * x1[0] + Rc[7] * x1[1] + Rc[8] * x1[2]};
-      // minimise | l1 a1 - l2 x2 + t |: normal equations of the 3 x 2 system [a1, -x2] (l1, l2)^T = -t
-      const double aa = a1[0] * a1[0] + a1[1] * a1[1] + a1[2] * a1[2];
-      const double bb = x2[0] * x2[0] + x2[1] * x2[1] + x2[2] * x2[2];
-      const double ab = a1[0] * x2[0] + a1[1] * x2[1] + a1[2] * x2[2];
-      const double at = a1[0] * tc[0] + a1[1] * tc[1] + a1[2] * tc[2];
-      const double bt = x2[0] * tc[0] + x2[1] * tc[1] + x2[2] * tc[2];
-      const double det = aa * bb - ab * ab;
-      const double l1 = (-at * bb + ab * bt) / det;
-      const double l2 = (aa * bt - ab * at) / det;
+      double l1, l2;
+      pose_depths(cand + 12 * c, cand + 12 * c + 9, x1, x2, &l1, &l2);
       if (l1 > 0 && l2 > 0) ++votes[c];
     }
   }
@@ -592,6 +607,199 @@ __global__ void pose_kernel(PoseArgs a) {
     for (int i = 0; i < 3; ++i) a.t[(size_t)p * 3 + i] = cand[12 * best + 9 + i];
     if (a.good) a.good[p] = votes[best];
   }
+}
+
+// ------------------------------------------------------------------------------------------------ pose from F, ragged
+constexpr int kPoseThreads = 256;     // = the 256 bins of the median's radix select: one bin per thread
+
+struct PoseRaggedArgs {
+  const double* F; const double* K1; const double* K2;   // [P][9] row-major; K: [9] shared or [P][9]
+  int k_per_pair;
+  const double* x1y1; const double* x2y2; const int* offsets; const unsigned char* mask;   // [rows][dim], [P+1], [rows]
+  int n_pairs, rows, dim;
+  double* R; double* t; int* good;                        // [P][9], [P][3], [P] (or null)
+  double* points; unsigned char* in_front; double* angle;   // [rows][3], [rows], [rows]
+  double* median;                                         // [P]
+};
+
+// Exclusive prefix of v over the CTA's threads (in thread order) and the CTA's total; ws: kPoseThreads / 32 ints.
+// Called by all threads; ends with a barrier after which ws may be reused.
+__device__ __forceinline__ int pose_block_scan(int v, int* ws, int* total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  int x = v;
+  for (int o = 1; o < 32; o <<= 1) {
+    const int y = __shfl_up_sync(0xffffffffu, x, o);
+    if (lane >= o) x += y;
+  }
+  if (lane == 31) ws[wid] = x;
+  __syncthreads();
+  int off = 0, tot = 0;
+  for (int w = 0; w < kPoseThreads / 32; ++w) { if (w < wid) off += ws[w]; tot += ws[w]; }
+  __syncthreads();
+  *total = tot;
+  return off + x - v;
+}
+
+// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1.
+//   pass 1: lane 0 of warp 0 builds the four candidates (pose_candidates), lane 1 the inverse calibrations;
+//   pass 2: the block votes over the rows with mask != 0 (pose_depths), first candidate wins ties -- the arithmetic and
+//           tie rule of pose_kernel, so R, t, good are those of a dense call on the pair alone;
+//   pass 3: per row under the chosen (R, t): in_front = mask && l1 > 0 && l2 > 0, the midpoint
+//           0.5 (l1 x1 + R^T (l2 x2 - t)) in camera 1's frame, the parallax angle atan2(|x1 x R^T x2|, x1 . R^T x2);
+//   pass 4: the median of the angles of the in-front rows, read back from global memory after a barrier: a radix
+//           select over the bit patterns of the (non-negative) doubles, eight 8-bit digits from the top, which needs no
+//           workspace and no bound on the row count.  An even count averages the two middle values as np.median does.
+// A pair whose F is all zero (no model) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, in_front = 0,
+// median NaN.  Offsets that decrease, are negative or pass `rows` make an empty pair: no row is read or written.
+__global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArgs a) {
+  __shared__ double cand[4 * 12];
+  __shared__ double kinv[18];
+  __shared__ int ws[kPoseThreads / 32];
+  __shared__ int wvotes[kPoseThreads / 32][4];
+  __shared__ unsigned hist[256];
+  __shared__ int s_best, s_digit, s_below, s_eq;
+  __shared__ unsigned long long s_min[kPoseThreads / 32];
+  const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int b = a.offsets[p], e = a.offsets[p + 1];
+  const bool span_ok = b >= 0 && b <= e && e <= a.rows;
+  const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
+  const double* F = a.F + (size_t)p * 9;
+  bool zero = true, has_nan = false;
+  for (int i = 0; i < 9; ++i) { zero &= F[i] == 0.0; has_nan |= F[i] != F[i]; }
+  if (zero || has_nan) {                          // (block-uniform)
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      for (int c = 0; c < 3; ++c) a.points[3 * r + c] = qnan();
+      a.in_front[r] = 0;
+      a.angle[r] = qnan();
+    }
+    if (tid < 9) a.R[(size_t)p * 9 + tid] = 0.0;
+    if (tid < 3) a.t[(size_t)p * 3 + tid] = 0.0;
+    if (tid == 0) {
+      if (a.good) a.good[p] = 0;
+      a.median[p] = qnan();
+    }
+    return;
+  }
+  const double* K1 = a.K1 + (a.k_per_pair ? (size_t)p * 9 : 0);
+  const double* K2 = a.K2 + (a.k_per_pair ? (size_t)p * 9 : 0);
+  if (tid == 0) pose_candidates(F, K1, K2, cand);
+  if (tid == 1) {                                 // the inverse calibrations (dg::inv3, as pose_kernel)
+    for (int i = 0; i < 9; ++i) { kinv[i] = K1[i]; kinv[9 + i] = K2[i]; }
+    dg::inv3(kinv);
+    dg::inv3(kinv + 9);
+  }
+  __syncthreads();
+
+  const unsigned char* mk = a.mask;
+  const double* g1 = a.x1y1;
+  const double* g2 = a.x2y2;
+  const int dim = a.dim;
+  int votes[4] = {0, 0, 0, 0};
+  for (int i = tid; i < n; i += kPoseThreads) {
+    const size_t r = (size_t)r0 + i;
+    if (mk && !mk[r]) continue;
+    double x1[3], x2[3];
+    pose_ray(kinv, g1[r * dim], g1[r * dim + 1], x1);
+    pose_ray(kinv + 9, g2[r * dim], g2[r * dim + 1], x2);
+    for (int c = 0; c < 4; ++c) {
+      double l1, l2;
+      pose_depths(cand + 12 * c, cand + 12 * c + 9, x1, x2, &l1, &l2);
+      if (l1 > 0 && l2 > 0) ++votes[c];
+    }
+  }
+  for (int c = 0; c < 4; ++c)
+    for (int o = 16; o > 0; o >>= 1) votes[c] += __shfl_xor_sync(0xffffffffu, votes[c], o);
+  if (lane == 0) for (int c = 0; c < 4; ++c) wvotes[wid][c] = votes[c];
+  __syncthreads();
+  if (tid == 0) {
+    int tot[4] = {0, 0, 0, 0};
+    for (int w = 0; w < kPoseThreads / 32; ++w) for (int c = 0; c < 4; ++c) tot[c] += wvotes[w][c];
+    int best = 0;
+    for (int c = 1; c < 4; ++c) if (tot[c] > tot[best]) best = c;
+    s_best = best;
+    wvotes[0][0] = tot[best];
+    if (a.good) a.good[p] = tot[best];
+  }
+  __syncthreads();
+  const int best = s_best, count = wvotes[0][0];
+  const double* Rb = cand + 12 * best;
+  const double* tb = Rb + 9;
+  if (tid < 9) a.R[(size_t)p * 9 + tid] = Rb[tid];
+  if (tid < 3) a.t[(size_t)p * 3 + tid] = tb[tid];
+
+  for (int i = tid; i < n; i += kPoseThreads) {
+    const size_t r = (size_t)r0 + i;
+    double x1[3], x2[3], l1, l2;
+    pose_ray(kinv, g1[r * dim], g1[r * dim + 1], x1);
+    pose_ray(kinv + 9, g2[r * dim], g2[r * dim + 1], x2);
+    pose_depths(Rb, tb, x1, x2, &l1, &l2);
+    a.in_front[r] = (!mk || mk[r]) && l1 > 0 && l2 > 0;
+    double y[3], q[3];                             // y = R^T x2, q = l2 x2 - t
+    for (int c = 0; c < 3; ++c) {
+      y[c] = Rb[c] * x2[0] + Rb[3 + c] * x2[1] + Rb[6 + c] * x2[2];
+      q[c] = l2 * x2[c] - tb[c];
+    }
+    for (int c = 0; c < 3; ++c)
+      a.points[3 * r + c] = 0.5 * (l1 * x1[c] + (Rb[c] * q[0] + Rb[3 + c] * q[1] + Rb[6 + c] * q[2]));
+    const double cx = x1[1] * y[2] - x1[2] * y[1], cy = x1[2] * y[0] - x1[0] * y[2], cz = x1[0] * y[1] - x1[1] * y[0];
+    a.angle[r] = atan2(sqrt(cx * cx + cy * cy + cz * cz), x1[0] * y[0] + x1[1] * y[1] + x1[2] * y[2]);
+  }
+  if (count == 0) {                                // (block-uniform)
+    if (tid == 0) a.median[p] = qnan();
+    return;
+  }
+  __syncthreads();                                 // this CTA's angle / in_front rows are visible to all its threads
+
+  // k-th smallest key (k = (count - 1) / 2) among the in-front rows: fix 8 bits per pass, from the top
+  int k = (count - 1) >> 1;
+  unsigned long long prefix = 0, known = 0;
+  for (int shift = 56; shift >= 0; shift -= 8) {
+    hist[tid] = 0;
+    __syncthreads();
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      if (!a.in_front[r]) continue;
+      const unsigned long long key = (unsigned long long)__double_as_longlong(a.angle[r]);
+      if ((key & known) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+    }
+    __syncthreads();
+    const int h = (int)hist[tid];
+    int tot;
+    const int below = pose_block_scan(h, ws, &tot);
+    if (below <= k && k < below + h) { s_digit = tid; s_below = below; s_eq = h; }
+    __syncthreads();
+    k -= s_below;
+    prefix |= (unsigned long long)s_digit << shift;
+    known |= 255ull << shift;
+  }
+  const double lo = __longlong_as_double((long long)prefix);
+  if (count & 1) {
+    if (tid == 0) a.median[p] = lo;
+    return;
+  }
+  // even count: the next order statistic is lo again when lo has further copies, else the smallest key above it
+  double hi = lo;
+  if (k + 1 >= s_eq) {                             // (block-uniform)
+    unsigned long long m = ~0ull;
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      if (!a.in_front[r]) continue;
+      const unsigned long long key = (unsigned long long)__double_as_longlong(a.angle[r]);
+      if (key > prefix && key < m) m = key;
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      const unsigned long long other = __shfl_xor_sync(0xffffffffu, m, o);
+      m = other < m ? other : m;
+    }
+    if (lane == 0) s_min[wid] = m;
+    __syncthreads();
+    if (tid == 0) {
+      for (int w = 1; w < kPoseThreads / 32; ++w) m = s_min[w] < m ? s_min[w] : m;
+      hi = __longlong_as_double((long long)m);
+    }
+  }
+  if (tid == 0) a.median[p] = (lo + hi) / 2.0;
 }
 
 // ------------------------------------------------------------------------------------------------ QR null space
@@ -879,6 +1087,26 @@ int dgb200_pose_from_fundamental_batch_dev(const double* d_F,const double* d_K1,
   a.n_pairs = n_pairs; a.n = n; a.dim = dim; a.R = d_R_out; a.t = d_t_out; a.good = d_good_out;
   const int threads = 256;
   pose_kernel<<<(n_pairs * 32 + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(a);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
+int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K1, const double* d_K2, int k_per_pair,
+                                            const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets,
+                                            int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                            double* d_R_out, double* d_t_out, int32_t* d_good_out,
+                                            double* d_points_out, uint8_t* d_in_front_out, double* d_angle_out,
+                                            double* d_median_angle_out, void* stream) {
+  if (!d_F || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_median_angle_out) return fail2(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x1y1 || !d_x2y2 || !d_points_out || !d_in_front_out || !d_angle_out))
+    return fail2(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  PoseRaggedArgs a;
+  a.F = d_F; a.K1 = d_K1; a.K2 = d_K2; a.k_per_pair = k_per_pair; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2;
+  a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs; a.rows = rows; a.dim = dim;
+  a.R = d_R_out; a.t = d_t_out; a.good = d_good_out; a.points = d_points_out; a.in_front = d_in_front_out;
+  a.angle = d_angle_out; a.median = d_median_angle_out;
+  pose_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
   CU2(cudaGetLastError());
   return 0;
 }

@@ -21,6 +21,10 @@ Many image pairs at once (one matcher call, one RANSAC launch, no host read in b
 Guided re-match with the models found (candidates: the train keypoints within px_th of the epipolar line / transfer):
 
     g = match_descriptors_guided(descs, pairs, kps, F, 1.0, guide="F")
+
+Relative pose, triangulated points and parallax angles of the ragged result, still without a host read:
+
+    pose = pose_from_fundamental_ragged(F, K1, K2, m.pts1, m.pts2, m.offsets, mask)
 """
 import collections
 import ctypes
@@ -33,6 +37,7 @@ kTQ = 32   # query descriptors per 2-NN work item (frontend.cu)
 
 BatchLayout = collections.namedtuple("BatchLayout", "tile_prefix row_prefix col_prefix capacity n_max")
 BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offsets n_max")
+RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angle median_angle")
 
 
 def batch_layout(counts, pairs):
@@ -182,6 +187,77 @@ def pose_from_fundamental(F, K1, K2, pts1, pts2, mask=None):
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return R, t, good
+
+
+def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
+    """pose_from_fundamental over a ragged batch, with the triangulated points and parallax angles of every row.
+
+    The inputs are what the ragged pipeline produces (match_descriptors_batch, then findFundamentalMatrixBatch with
+    offsets=), all CUDA tensors on one device: F [P,3,3] or [P,9] (x2^T F x1 = 0), K1 / K2 [3,3] or [P,3,3], pts1 /
+    pts2 [rows, 2|6] (columns 0-1 are the pixel coordinates), offsets int32 [P+1] (pair p owns rows
+    offsets[p] .. offsets[p+1]-1), mask [rows] bool / uint8 or None (every row).  Floating inputs are used in float64.
+    Per pair, R, t and good are what pose_from_fundamental returns for the pair alone.  Per row, under the chosen pose:
+    points [rows,3] the midpoint of the two rays' closest points, in camera 1's frame and units of the baseline
+    (|t| = 1); in_front [rows] bool, mask and both depths positive (good is the pair's count of it); angle [rows] the
+    parallax angle between the rays in radians.  median_angle [P] is the median angle of the pair's in-front rows (NaN
+    when there is none): COLMAP-style tools keep pairs whose median parallax is large enough.  A pair whose F is all zero
+    (no model found) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, no in-front row and a NaN median.
+    Returns RaggedPose(R, t, good, points, in_front, angle, median_angle); asynchronous, nothing is read back."""
+    import torch
+    named = (("F", F), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
+    for name, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % name)
+    if F.dim() not in (2, 3) or F.shape[0] < 1 or tuple(F.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("F must be [P,3,3] or [P,9] with P >= 1, not %s" % list(F.shape))
+    P = int(F.shape[0])
+    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
+        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
+    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
+    for name, K in (("K1", K1), ("K2", K2)):
+        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
+            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (name, P, list(K.shape)))
+    if tuple(offsets.shape) != (P + 1,):
+        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
+    if offsets.dtype != torch.int32:
+        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
+    for name, x in (("F", F), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (rows,):
+            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    dev = pts1.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("F, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device")
+    per_pair = K1.dim() == 3 or K2.dim() == 3
+    if per_pair:
+        K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    f64 = torch.float64
+    Fc, K1c, K2c = (x.to(f64).contiguous() for x in (F, K1, K2))
+    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
+    off = offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        R = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        t = torch.empty((P, 3), dtype=f64, device=dev)
+        good = torch.empty(P, dtype=torch.int32, device=dev)
+        points = torch.empty((rows, 3), dtype=f64, device=dev)
+        in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
+        angle = torch.empty(rows, dtype=f64, device=dev)
+        median = torch.empty(P, dtype=f64, device=dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_pose_from_fundamental_ragged_dev(
+            vp(Fc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), int(per_pair), vp(p1.data_ptr()),
+            vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim, vp(m.data_ptr()) if m is not None else None,
+            vp(R.data_ptr()), vp(t.data_ptr()), vp(good.data_ptr()), vp(points.data_ptr()), vp(in_front.data_ptr()),
+            vp(angle.data_ptr()), vp(median.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_frontend_last_error().decode())
+    return RaggedPose(R, t, good, points, in_front.view(torch.bool), angle, median)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
