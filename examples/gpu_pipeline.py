@@ -5,6 +5,7 @@
                                             ->  findHomography / findFundamentalMatrix (device-resident tensors)
                                             ->  guided re-match inside F's epipolar band   (pydegensac_b200.matching, CUDA)
                                             ->  relative pose from F                      (pydegensac_b200.matching)
+                                            ->  pose refined on the inliers (Sampson error) (pydegensac_b200.matching)
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -20,7 +21,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import match_descriptors, match_descriptors_guided, pose_from_fundamental
+from pydegensac_b200.matching import (match_descriptors, match_descriptors_guided, pose_from_fundamental,
+                                      pose_from_fundamental_ragged, refine_pose_ragged)
 from pydegensac_b200.scenes import scene_F, _K
 
 
@@ -51,6 +53,13 @@ def main():
     K = torch.from_numpy(_K).to(dev)
     R, t, good = pose_from_fundamental(F, K, K, pts1[None], pts2[None], mask)
     print("R =\n", R[0].cpu().numpy(), "\nt =", t[0].cpu().numpy(), " (%d correspondences in front of both cameras)" % int(good[0]))
+    # refinement on the inliers in front of both cameras, through the ragged entry points with one pair
+    offsets = torch.tensor([0, len(idx1)], dtype=torch.int32, device=dev)
+    pose = pose_from_fundamental_ragged(F, K, K, pts1, pts2, offsets, mask[0])
+    fine = refine_pose_ragged(pose.R, pose.t, K, K, pts1, pts2, offsets, pose.in_front, px_th=0.5)
+    print("refined on %d rows in %d trial steps: sum of squared Sampson residuals %.3f -> %.3f px^2, %d inliers at 0.5 px"
+          % (int(fine.n_used[0]), int(fine.iters[0]), float(fine.cost0[0]), float(fine.cost[0]), int(fine.inliers.sum())))
+    print("R =\n", fine.R[0].cpu().numpy(), "\nt =", fine.t[0].cpu().numpy())
 
 
 if __name__ == "__main__":

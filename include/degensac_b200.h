@@ -270,6 +270,36 @@ int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K
                                             double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                             double* d_points_out, uint8_t* d_in_front_out, double* d_angle_out,
                                             double* d_median_angle_out, void* stream);
+/* Refinement of the relative pose on the inliers, over a RAGGED batch laid out as above (d_offsets, d_x1y1 / d_x2y2,
+ * d_mask, K): per pair, Levenberg-Marquardt from (d_R [n_pairs][9] row-major, d_t [n_pairs][3] of unit length; what
+ * dgb200_pose_from_fundamental_ragged_dev returns) on the cost C(R, t) = sum of r^2 over the rows with mask != 0, r the
+ * pixel-domain Sampson residual of F = K2^-T [t]x R K1^-1, so r^2 is the residual of the RANSAC's inlier rule (px^2).
+ * Five local parameters, re-centred at every accepted step: R <- exp([w]x) R, t <- (t + B d) / |t + B d| with B an
+ * orthonormal basis of the plane orthogonal to t; analytic Jacobian.  Schedule: lambda = 1e-3; a trial step solves
+ * (J^T J + lambda diag(J^T J)) D = -J^T r (a pivot of the 5 x 5 Cholesky factor that is not positive rejects it) and is
+ * accepted when its cost is strictly lower (lambda <- max(lambda / 10, 1e-12)), else lambda <- 10 lambda; stops after
+ * max_iters trial steps, after a trial step, accepted or not, whose cost differs from the current one by less than
+ * 1e-12 of it (converged), or when lambda > 1e8.
+ * The sums of a pair are reduced in a fixed order without atomics: its result does not depend on the batch or the run.
+ * Outputs per pair: d_R_out [9], d_t_out [3] (det R = +1, |t| = 1); d_F_out [9] = K2^-T [t]x R K1^-1 row-major, scaled
+ * to unit Frobenius norm (x2^T F x1 = 0: the model dgb200_match_descriptors_guided_batch_dev takes); d_cost0_out,
+ * d_cost_out the cost before and after (cost <= cost0); d_n_used_out the rows with mask != 0; d_iters_out the trial
+ * steps taken.  d_inliers_out [rows], when given: f_resid_sampson(F, row) <= px_th^2 with the output F for EVERY row of
+ * the pair, masked or not -- the comparison of the RANSAC's mask.
+ * Pairs that are not refined: fewer than 6 rows with mask != 0: R, t copied, F built from them, cost0 = cost = their
+ * cost, iters = 0.  R all zero, or a NaN in R or t (no model): R = t = F = 0, NaN costs, n_used = iters = 0, inlier rows
+ * 0.  Offsets that decrease, are negative or pass `rows`: per-pair outputs as for no model, no row read or written.
+ * d_mask, d_cost0_out, d_n_used_out, d_iters_out and d_inliers_out may be NULL; d_x1y1 / d_x2y2 may be NULL when
+ * rows = 0; every other buffer is required.  d_R_out / d_t_out may be d_R / d_t (in place).  A null required buffer,
+ * n_pairs < 1, rows < 0, dim < 2, max_iters < 0, or d_inliers_out with a negative or NaN px_th returns DGB200_E_ARG
+ * before any launch.  Asynchronous on `stream`, one kernel, no workspace. */
+int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const double* d_K1, const double* d_K2,
+                                  int k_per_pair, const double* d_x1y1, const double* d_x2y2,
+                                  const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                  int max_iters, double px_th,
+                                  double* d_R_out, double* d_t_out, double* d_F_out, double* d_cost0_out,
+                                  double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                  uint8_t* d_inliers_out, void* stream);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

@@ -22,6 +22,7 @@
 #include "common.h"
 #include "la.h"
 #include "hgeom.h"
+#include "pose_refine.h"
 #include "rng.h"
 
 namespace {
@@ -802,6 +803,180 @@ __global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArg
   if (tid == 0) a.median[p] = (lo + hi) / 2.0;
 }
 
+// ------------------------------------------------------------------------------------------------ pose refinement, ragged
+struct PoseRefineArgs {
+  const double* R; const double* t; const double* K1; const double* K2;   // [P][9], [P][3]; K: [9] shared or [P][9]
+  int k_per_pair;
+  const double* x1y1; const double* x2y2; const int* offsets; const unsigned char* mask;   // [rows][dim], [P+1], [rows]
+  int n_pairs, rows, dim, max_iters;
+  double th2;                                              // px_th^2 of the inlier rows
+  double* R_out; double* t_out; double* F_out;             // [P][9], [P][3], [P][9]
+  double* cost0; double* cost; int* n_used; int* iters;    // [P] (cost0, n_used, iters may be null)
+  unsigned char* inliers;                                  // [rows] or null
+};
+
+// One pass over the pair's rows with mask != 0 at the linearisation (F, dF) in shared memory: the cost, J^T J and J^T r
+// (dg::pr_row) summed over the CTA into out[kPrSums], the number of rows into *count.  A fixed-shape tree: butterfly
+// shuffles inside each warp, then thread j < kPrSums adds the warps' partials of sum j in warp order -- no atomics, so
+// the sums of a pair do not depend on the batch it is in or on the run.  Called by all threads; ends with a barrier.
+__device__ __forceinline__ void pose_refine_pass(const PoseRefineArgs& a, int r0, int n, const double* F, const double* dF,
+                                                 double (*wpart)[dg::kPrSums], int* wcount, double* out, int* count) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const unsigned char* mk = a.mask;
+  const double* g1 = a.x1y1;
+  const double* g2 = a.x2y2;
+  const int dim = a.dim;
+  double acc[dg::kPrSums];
+#pragma unroll
+  for (int j = 0; j < dg::kPrSums; ++j) acc[j] = 0.0;
+  int cnt = 0;
+  for (int i = tid; i < n; i += kPoseThreads) {
+    const size_t r = (size_t)r0 + i;
+    if (mk && !mk[r]) continue;
+    ++cnt;
+    dg::pr_row(F, dF, g1[r * dim], g1[r * dim + 1], g2[r * dim], g2[r * dim + 1], acc);
+  }
+#pragma unroll
+  for (int j = 0; j < dg::kPrSums; ++j)
+    for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) {
+#pragma unroll
+    for (int j = 0; j < dg::kPrSums; ++j) wpart[wid][j] = acc[j];
+    wcount[wid] = cnt;
+  }
+  __syncthreads();
+  if (tid < dg::kPrSums) {
+    double s = wpart[0][tid];
+    for (int w = 1; w < kPoseThreads / 32; ++w) s += wpart[w][tid];
+    out[tid] = s;
+  } else if (tid == dg::kPrSums) {
+    int c = 0;
+    for (int w = 0; w < kPoseThreads / 32; ++w) c += wcount[w];
+    *count = c;
+  }
+  __syncthreads();
+}
+
+// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1: Levenberg-Marquardt with Marquardt scaling on the
+// Sampson cost C(R, t) = sum of f_resid_sampson over the rows with mask != 0, from the pose given (pose_refine.h has the
+// residual, its analytic Jacobian and the local parameters).
+//   start:  thread 0 linearises at (R, t); one pass gives C, H = J^T J, g = J^T r there; lambda = 1e-3.
+//   trial:  thread 0 solves (H + lambda diag H) D = -g (5 x 5 Cholesky; a pivot that is not positive rejects the step
+//           without a pass), moves to the trial pose and linearises there; one pass gives the trial C', H', g'.
+//           C' < C: the trial pose and its sums become current, lambda <- max(lambda / 10, 1e-12).  Otherwise the
+//           current sums stay, lambda <- 10 lambda, stop when lambda > 1e8.  Either way |C - C'| < 1e-12 C stops the
+//           refinement: at the minimum a trial step moves the cost by rounding only, up as often as down.
+//   So k trial steps read the rows at most k + 1 times, from global memory (a pair's rows stay in L2).
+//   end:    R re-orthonormalised if an accepted step left |R R^T - I| above 1e-12; F = K2^-T [t]x R K1^-1 scaled to unit
+//           Frobenius norm; with inliers_out one more pass over ALL the pair's rows: f_resid_sampson(F, ..) <= th2.
+// Fewer than kPrMinRows rows with mask != 0: the pose is passed through, cost0 = cost = its cost, iters = 0.  R all zero
+// or a NaN in R or t (no model): R = t = F = 0, NaN costs, n_used = iters = 0, inlier rows 0.  Offsets that decrease, are
+// negative or pass `rows`: the same per-pair outputs and no row is read or written.  R_out / t_out may be R / t: the
+// pose is read into shared memory before the first barrier and written after it.
+__global__ void __launch_bounds__(kPoseThreads) pose_refine_ragged_kernel(PoseRefineArgs a) {
+  __shared__ double kinv[18];                      // K1^-1, K2^-1
+  __shared__ double kA[9];                         // K2^-T
+  __shared__ double pose[2][12];                   // current and trial (R [9], t [3])
+  __shared__ double lin[54];                       // F [9], dF [5][9] of the pass to come; at the end the output F
+  __shared__ double cur[dg::kPrSums], trial[dg::kPrSums];
+  __shared__ double wpart[kPoseThreads / 32][dg::kPrSums];
+  __shared__ int wcount[kPoseThreads / 32];
+  __shared__ int s_count, s_go;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int b = a.offsets[p], e = a.offsets[p + 1];
+  const bool span_ok = b >= 0 && b <= e && e <= a.rows;
+  const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
+  if (tid < 9) pose[0][tid] = a.R[(size_t)p * 9 + tid];
+  else if (tid < 12) pose[0][tid] = a.t[(size_t)p * 3 + tid - 9];
+  __syncthreads();                                 // the pose is read: the outputs may overwrite it
+  bool zero = true, has_nan = false;
+  for (int i = 0; i < 12; ++i) { zero &= i >= 9 || pose[0][i] == 0.0; has_nan |= pose[0][i] != pose[0][i]; }
+  if (!span_ok || zero || has_nan) {               // (block-uniform)
+    if (a.inliers) for (int i = tid; i < n; i += kPoseThreads) a.inliers[(size_t)r0 + i] = 0;
+    if (tid < 9) { a.R_out[(size_t)p * 9 + tid] = 0.0; a.F_out[(size_t)p * 9 + tid] = 0.0; }
+    if (tid < 3) a.t_out[(size_t)p * 3 + tid] = 0.0;
+    if (tid == 0) {
+      a.cost[p] = qnan();
+      if (a.cost0) a.cost0[p] = qnan();
+      if (a.n_used) a.n_used[p] = 0;
+      if (a.iters) a.iters[p] = 0;
+    }
+    return;
+  }
+  if (tid == 0) {                                  // the inverse calibrations (dg::inv3, as the pose kernels)
+    const double* K1 = a.K1 + (a.k_per_pair ? (size_t)p * 9 : 0);
+    const double* K2 = a.K2 + (a.k_per_pair ? (size_t)p * 9 : 0);
+    for (int i = 0; i < 9; ++i) { kinv[i] = K1[i]; kinv[9 + i] = K2[i]; }
+    dg::inv3(kinv);
+    dg::inv3(kinv + 9);
+    for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) kA[3 * i + j] = kinv[9 + 3 * j + i];
+    dg::pr_linearise(pose[0], pose[0] + 9, kA, kinv, lin, lin + 9);
+  }
+  __syncthreads();
+  pose_refine_pass(a, r0, n, lin, lin + 9, wpart, wcount, cur, &s_count);
+  const int n_used = s_count;
+  const double cost0 = cur[0];
+  double lam = dg::kPrLambda0;
+  int iters = 0, accepted = 0;
+  while (n_used >= dg::kPrMinRows && iters < a.max_iters) {   // (block-uniform: every thread keeps the same lam, iters)
+    ++iters;
+    if (tid == 0) {
+      double D[5];
+      s_go = dg::pr_solve(cur + 1, cur + 16, lam, D) ? 1 : 0;
+      if (s_go) {
+        dg::pr_step(pose[0], pose[0] + 9, D, pose[1], pose[1] + 9);
+        dg::pr_linearise(pose[1], pose[1] + 9, kA, kinv, lin, lin + 9);
+      }
+    }
+    __syncthreads();
+    const bool go = s_go != 0;
+    if (go) pose_refine_pass(a, r0, n, lin, lin + 9, wpart, wcount, trial, &s_count);
+    const double c_old = cur[0], c_new = trial[0];
+    const bool better = go && c_new < c_old;
+    const bool flat = go && fabs(c_old - c_new) < dg::kPrRelDecrease * c_old;   // converged: the cost no longer moves
+    __syncthreads();                               // s_go, cur[0], trial[0] are read: they may change
+    if (better) {
+      if (tid < dg::kPrSums) cur[tid] = trial[tid];
+      if (tid < 12) pose[0][tid] = pose[1][tid];
+    }
+    __syncthreads();
+    if (better) {
+      lam = fmax(lam / 10.0, dg::kPrLambdaMin);
+      ++accepted;
+      if (flat) break;
+    } else {
+      lam *= 10.0;
+      if (flat || lam > dg::kPrLambdaMax) break;
+    }
+  }
+  if (tid == 0) {
+    if (accepted && dg::pr_ortho_drift(pose[0]) > dg::kPrOrthoTol) dg::pr_orthonormalise(pose[0]);
+    double F[9];
+    dg::pr_fundamental(pose[0], pose[0] + 9, kA, kinv, F);
+    double nrm = 0.0;
+    for (int i = 0; i < 9; ++i) nrm += F[i] * F[i];
+    const double inv = nrm > 0.0 ? 1.0 / sqrt(nrm) : 0.0;
+    for (int i = 0; i < 9; ++i) lin[i] = F[i] * inv;
+  }
+  __syncthreads();
+  if (tid < 9) { a.R_out[(size_t)p * 9 + tid] = pose[0][tid]; a.F_out[(size_t)p * 9 + tid] = lin[tid]; }
+  if (tid < 3) a.t_out[(size_t)p * 3 + tid] = pose[0][9 + tid];
+  if (tid == 0) {
+    a.cost[p] = cur[0];
+    if (a.cost0) a.cost0[p] = cost0;
+    if (a.n_used) a.n_used[p] = n_used;
+    if (a.iters) a.iters[p] = iters;
+  }
+  if (a.inliers) {
+    const int dim = a.dim;
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      a.inliers[r] = dg::f_resid_sampson(lin, a.x1y1[r * dim], a.x1y1[r * dim + 1], a.x2y2[r * dim], a.x2y2[r * dim + 1]) <= a.th2;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ QR null space
 __global__ void qr7x9_kernel(const double* A, double* N, int* rc, int count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1107,6 +1282,29 @@ int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K
   a.R = d_R_out; a.t = d_t_out; a.good = d_good_out; a.points = d_points_out; a.in_front = d_in_front_out;
   a.angle = d_angle_out; a.median = d_median_angle_out;
   pose_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
+int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const double* d_K1, const double* d_K2,
+                                  int k_per_pair, const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets,
+                                  int n_pairs, int rows, int dim, const uint8_t* d_mask, int max_iters, double px_th,
+                                  double* d_R_out, double* d_t_out, double* d_F_out, double* d_cost0_out,
+                                  double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                  uint8_t* d_inliers_out, void* stream) {
+  if (!d_R || !d_t || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_F_out || !d_cost_out)
+    return fail2(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
+  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+  PoseRefineArgs a;
+  a.R = d_R; a.t = d_t; a.K1 = d_K1; a.K2 = d_K2; a.k_per_pair = k_per_pair; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2;
+  a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs; a.rows = rows; a.dim = dim; a.max_iters = max_iters;
+  a.th2 = d_inliers_out ? px_th * px_th : 0.0;
+  a.R_out = d_R_out; a.t_out = d_t_out; a.F_out = d_F_out; a.cost0 = d_cost0_out; a.cost = d_cost_out;
+  a.n_used = d_n_used_out; a.iters = d_iters_out; a.inliers = d_inliers_out;
+  pose_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
   CU2(cudaGetLastError());
   return 0;
 }

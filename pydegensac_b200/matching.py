@@ -25,6 +25,10 @@ Guided re-match with the models found (candidates: the train keypoints within px
 Relative pose, triangulated points and parallax angles of the ragged result, still without a host read:
 
     pose = pose_from_fundamental_ragged(F, K1, K2, m.pts1, m.pts2, m.offsets, mask)
+
+The pose refined on its inliers (Levenberg-Marquardt on the Sampson error), with the calibrated F for a guided re-match:
+
+    fine = refine_pose_ragged(pose.R, pose.t, K1, K2, m.pts1, m.pts2, m.offsets, pose.in_front)
 """
 import collections
 import ctypes
@@ -38,6 +42,7 @@ kTQ = 32   # query descriptors per 2-NN work item (frontend.cu)
 BatchLayout = collections.namedtuple("BatchLayout", "tile_prefix row_prefix col_prefix capacity n_max")
 BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offsets n_max")
 RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angle median_angle")
+RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used iters inliers")
 
 
 def batch_layout(counts, pairs):
@@ -258,6 +263,93 @@ def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return RaggedPose(R, t, good, points, in_front.view(torch.bool), angle, median)
+
+
+def refine_pose_ragged(R, t, K1, K2, pts1, pts2, offsets, mask=None, max_iters=10, px_th=None):
+    """Refine the relative pose of every pair of a ragged batch on its inliers: Levenberg-Marquardt on the Sampson error.
+
+    pose_from_fundamental_ragged takes its pose from an uncalibrated F; this step minimises, per pair, the sum of the
+    squared pixel-domain Sampson residuals of F = K2^-T [t]x R K1^-1 over the rows with mask set -- the residual of the
+    RANSAC's inlier rule -- over the five degrees of freedom of (R, t), |t| = 1, starting from the pose given.
+    All inputs are CUDA tensors on one device: R [P,3,3] or [P,9], t [P,3] (x2 ~ R x1 + t), K1 / K2 [3,3] or [P,3,3],
+    pts1 / pts2 [rows, 2|6], offsets int32 [P+1], mask [rows] bool / uint8 or None (every row), as
+    pose_from_fundamental_ragged takes and returns them; floating inputs are used in float64.  The intended call is
+    refine_pose_ragged(pose.R, pose.t, K1, K2, m.pts1, m.pts2, m.offsets, pose.in_front): the RANSAC's inliers that
+    triangulate in front of both cameras.  max_iters bounds the trial steps per pair (schedule: include/degensac_b200.h).
+    Returns RefinedPose(R, t, F, cost0, cost, n_used, iters, inliers): R [P,3,3], t [P,3] refined; F [P,3,3] the
+    calibrated fundamental matrix of (R, t), unit Frobenius norm (x2^T F x1 = 0), the model match_descriptors_guided(...,
+    guide="F") takes; cost0 / cost [P] the sum of squared residuals (px^2) before and after, cost <= cost0; n_used [P]
+    int32 the rows used; iters [P] int32 the trial steps taken; inliers [rows] bool, with px_th given: Sampson residual
+    of the refined F at most px_th^2 for every row, masked or not (None without px_th).  A pair with fewer than 6 rows
+    used keeps its pose (iters 0); a pair whose R is all zero or holds a NaN (no model) gets R = t = F = 0, NaN costs and
+    no inliers.  The result of a pair does not depend on the batch it is in.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("R", R), ("t", t), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
+    for name, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % name)
+    if R.dim() not in (2, 3) or R.shape[0] < 1 or tuple(R.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("R must be [P,3,3] or [P,9] with P >= 1, not %s" % list(R.shape))
+    P = int(R.shape[0])
+    if tuple(t.shape) != (P, 3):
+        raise ValueError("t must be [P,3] = [%d,3], not %s" % (P, list(t.shape)))
+    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
+        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
+    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
+    for name, K in (("K1", K1), ("K2", K2)):
+        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
+            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (name, P, list(K.shape)))
+    if tuple(offsets.shape) != (P + 1,):
+        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
+    if offsets.dtype != torch.int32:
+        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
+    for name, x in (("R", R), ("t", t), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (rows,):
+            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    max_iters = int(max_iters)
+    if max_iters < 0:
+        raise ValueError("max_iters must not be negative, not %d" % max_iters)
+    if px_th is not None:
+        px_th = float(px_th)
+        if not px_th >= 0.0:
+            raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
+    dev = pts1.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("R, t, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device")
+    per_pair = K1.dim() == 3 or K2.dim() == 3
+    if per_pair:
+        K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    f64 = torch.float64
+    Rc, tc, K1c, K2c = (x.to(f64).contiguous() for x in (R, t, K1, K2))
+    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
+    off = offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        Ro = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        to = torch.empty((P, 3), dtype=f64, device=dev)
+        Fo = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        cost0 = torch.empty(P, dtype=f64, device=dev)
+        cost = torch.empty(P, dtype=f64, device=dev)
+        n_used = torch.empty(P, dtype=torch.int32, device=dev)
+        iters = torch.empty(P, dtype=torch.int32, device=dev)
+        inl = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows] if px_th is not None else None
+        vp = ctypes.c_void_p
+        rc = L.dgb200_refine_pose_ragged_dev(
+            vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), int(per_pair),
+            vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
+            vp(m.data_ptr()) if m is not None else None, max_iters, ctypes.c_double(px_th if px_th is not None else 0.0),
+            vp(Ro.data_ptr()), vp(to.data_ptr()), vp(Fo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()),
+            vp(n_used.data_ptr()), vp(iters.data_ptr()), vp(inl.data_ptr()) if inl is not None else None,
+            vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_frontend_last_error().decode())
+    return RefinedPose(Ro, to, Fo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
