@@ -50,8 +50,10 @@ int cfg_chunk() {   // iterations hypothesised per wave (DGB200_CHUNK, multiple 
 #define kChunk cfg_chunk()
 
 // CTA shape.  256 threads x 2 CTAs per SM measured fastest on H100 (profiles/README.md; one CTA per SM: -27 %): the waves and the O(N)
-// passes of the replay want the 8 warps, while more, smaller CTAs per SM lose to instruction-cache misses (each
-// CTA walks a different part of a ~300 KB code image).  FP64 correspondences live in the per-CTA global slab
+// passes of the replay want the 8 warps.  More, narrower CTAs at the same 128 registers per thread are slower on
+// config 2 (160 x 3: -6.6 %, 128 x 4: -13 % to -21 %; profiles/h100_cta_width.txt): on half the warps the O(N) passes
+// take over twice as long, and the extra resident pairs (each walking a different part of a ~300 KB code image)
+// do not hide that.  FP64 correspondences live in the per-CTA global slab
 // (L1/L2 resident), the FP32 filter tile in shared memory.  DGB200_THREADS / DGB200_SMEM_TILE override for experiments.
 int cfg_threads() {
   static int v = -1;
@@ -257,6 +259,7 @@ struct Cache {
   int device = -1;
   int sm_count = 0;
   size_t smem_optin = 0;
+  size_t smem_per_sm = 0, smem_reserved = 0;   // shared memory per SM at the largest carveout; reserved per CTA
   std::vector<LaunchCtx> ctxs;
   unsigned char* io = nullptr; size_t io_bytes = 0;   // staging for the host-buffer flavour
   cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev_feed = nullptr;
@@ -312,6 +315,8 @@ int ensure_device() {
   Cache c;
   c.sm_count = prop.multiProcessorCount;
   c.smem_optin = prop.sharedMemPerBlockOptin;
+  c.smem_per_sm = prop.sharedMemPerMultiprocessor;
+  c.smem_reserved = prop.reservedSharedMemPerBlock;
   cudaError_t err = cudaSuccess;
   auto step = [&](cudaError_t r) { if (err == cudaSuccess) err = r; };
   step(cudaEventCreate(&c.ev0));
@@ -386,6 +391,8 @@ int launch(const Job& j, cudaStream_t st, const int* d_ready = nullptr, int* d_s
   const size_t tile32 = (16 * ((size_t)n + 1) <= 98304) ? dg::align_up(16 * ((size_t)n + 1), 128) * kGroups : 0;   // FP32 filter tile(s) (pair-interleaved: N+1 slots)
   const int kThreads = (kGroups > 1) ? 32 * DG_CTA_WARPS : cfg_threads();
   auto kern = ransac_pairs_kernel<KIND>;
+  // the occupancy queries below see the driver's own carveout choice (a previous launch may have narrowed it)
+  CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutDefault));
   // Shared-memory plan: block scratch always; the FP32 filter tile when it fits.  The FP64 correspondences stay in
   // global memory (L1/L2-resident): DGB200_SMEM_TILE=1 moves them to shared memory too, at the cost of the L1 capacity
   // the residual rows and lists live in.
@@ -419,6 +426,20 @@ int launch(const Job& j, cudaStream_t st, const int* d_ready = nullptr, int* d_s
   if (!a.pts_in_smem) {
     CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kThreads, smem));
+    if (KIND == 0 && per_sm >= 1 && g_c.smem_per_sm > 0) {
+      // L1 and shared memory split one 256 KB array per SM.  The driver's default split leaves the F kernel less L1 than
+      // it can have; ask for the smallest carveout that still holds the same CTAs per SM (2 x 16 KB of block scratch:
+      // the 64 KB configuration, 192 KB of L1).  The serial steps' stack, lists and hypothesis queue live in L1:
+      // config 2 on H100 +4 % (profiles/h100_carveout.txt).  Results do not depend on it.
+      const size_t need = (size_t)per_sm * (smem + g_c.smem_reserved);
+      int pct = (int)((100 * need + g_c.smem_per_sm - 1) / g_c.smem_per_sm);
+      if (pct > 100) pct = 100;
+      CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+      int occ = 0;
+      CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, kThreads, smem));
+      if (occ < per_sm)   // the split the driver picks from the hint must not cost a resident CTA
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, (int)cudaSharedmemCarveoutDefault));
+    }
   }
   if (per_sm < 1) return fail(DGB200_E_CUDA, "kernel does not fit on an SM");
   { const int cap = env_int("DGB200_CTAS_PER_SM", 0); if (cap >= 1 && cap < per_sm) per_sm = cap; }
