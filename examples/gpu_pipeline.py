@@ -6,6 +6,7 @@
                                             ->  guided re-match inside F's epipolar band   (pydegensac_b200.matching, CUDA)
                                             ->  relative pose from F                      (pydegensac_b200.matching)
                                             ->  pose refined on the inliers (Sampson error) (pydegensac_b200.matching)
+    and the H branch for a planar scene:    ->  findHomographyBatch -> pose and scene plane from H
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -22,8 +23,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
 from pydegensac_b200.matching import (match_descriptors, match_descriptors_guided, pose_from_fundamental,
-                                      pose_from_fundamental_ragged, refine_pose_ragged)
-from pydegensac_b200.scenes import scene_F, _K
+                                      pose_from_fundamental_ragged, pose_from_homography_ragged, refine_pose_ragged)
+from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
 def synth_features(n_true=1200, n_clutter=800, D=64, seed=0):
@@ -37,6 +38,17 @@ def synth_features(n_true=1200, n_clutter=800, D=64, seed=0):
     d2 = np.r_[base + 0.2 * rng.normal(size=base.shape).astype(np.float32), rng.normal(size=(n_clutter, D)).astype(np.float32)]
     perm = rng.permutation(len(kp2))
     return kp1, d1, kp2[perm], d2[perm]
+
+
+def synth_plane(n=1000, seed=1):
+    """Two views of points on a plane (a facade 6 units away, tilted): pixel pairs with 0.3 px noise."""
+    rng = np.random.default_rng(seed)
+    R, t = _rot("y", -0.15) @ _rot("x", 0.05), np.array([1.0, 0.1, 0.2])
+    nrm = np.array([0.2, -0.1, 1.0]) / np.linalg.norm([0.2, -0.1, 1.0])
+    xy = np.c_[rng.uniform(-3, 3, n), rng.uniform(-2, 2, n)]
+    X = np.c_[xy, (6.0 - xy @ nrm[:2]) / nrm[2]]
+    x1, x2 = X @ _K.T, (X @ R.T + t) @ _K.T
+    return (x1[:, :2] / x1[:, 2:3] + 0.3 * rng.normal(size=(n, 2)), x2[:, :2] / x2[:, 2:3] + 0.3 * rng.normal(size=(n, 2)))
 
 
 def main():
@@ -60,6 +72,16 @@ def main():
     print("refined on %d rows in %d trial steps: sum of squared Sampson residuals %.3f -> %.3f px^2, %d inliers at 0.5 px"
           % (int(fine.n_used[0]), int(fine.iters[0]), float(fine.cost0[0]), float(fine.cost[0]), int(fine.inliers.sum())))
     print("R =\n", fine.R[0].cpu().numpy(), "\nt =", fine.t[0].cpu().numpy())
+    # the H branch: a planar scene, where F is not determined; pose and plane from H, the two best decompositions
+    q1, q2 = (torch.from_numpy(a).to(dev) for a in synth_plane())
+    qoff = torch.tensor([0, len(q1)], dtype=torch.int32, device=dev)
+    H, hmask = pydegensac.findHomographyBatch(q1, q2, 2.0, 0.999, 10000, seeds=[0], offsets=qoff, n_max=len(q1))
+    hp = pose_from_homography_ragged(H, K, K, q1, q2, qoff, hmask)
+    for c, name in enumerate(("chosen", "runner-up")):
+        print("H branch, %s pose (%d votes): R =\n" % (name, int(hp.good[0, c])), hp.R[0, c].cpu().numpy(),
+              "\nt =", hp.t[0, c].cpu().numpy(), " plane n =", hp.plane[0, c, :3].cpu().numpy(),
+              " d = %.3f" % float(hp.plane[0, c, 3]))
+    print("median parallax of the chosen pose: %.2f deg" % np.degrees(float(hp.median_angle[0])))
 
 
 if __name__ == "__main__":

@@ -270,6 +270,42 @@ int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K
                                             double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                             double* d_points_out, uint8_t* d_in_front_out, double* d_angle_out,
                                             double* d_median_angle_out, void* stream);
+/* Pose and scene plane from homographies over a RAGGED batch laid out as above (d_offsets, d_x1y1 / d_x2y2, d_mask,
+ * K), for planar scenes and pure rotations, where F is undetermined or does not exist.  d_H [n_pairs][9] row-major,
+ * x2 ~ H x1 (OpenCV convention, what dgb200_find_homography_* return).  Per pair, in FP64:
+ *   Hn = K2^-1 H K1 divided by its middle singular value, negated when det(Hn) < 0;
+ *   max |(Hn^T Hn - I)_ij| < 1e-3: a PURE ROTATION, one candidate R = U V^T (the rotation nearest to Hn), t = 0;
+ *   otherwise the four decompositions Hn = R + t' n^T, |n| = 1, of Malis & Vargas (INRIA RR-6303, the analytical
+ *   method, as cv2.decomposeHomographyMat) in the order (Ra, t'a, na), (Ra, -t'a, -na), (Rb, t'b, nb), (Rb, -t'b, -nb).
+ * Vote over the rows with mask != 0: a row supports (R, t'/|t'|) when the least-squares depths (l1, l2) of
+ * l1 R x1 + t = l2 x2 are both positive (the arithmetic of the F entry points), the rotation when x1 . R^T x2 > 0.
+ * Candidate 0 has the most votes, candidate 1 the most among the rest; equal votes go to the earlier candidate in the
+ * order above.  Two views of a plane often leave two candidates with equal votes: candidate 1 is the one a caller with
+ * a prior (the ground-plane normal, a third view) may prefer.  Outputs, for c = 0, 1:
+ *   d_R_out [n_pairs][2][9]      row-major, det R = +1;
+ *   d_t_out [n_pairs][2][3]      unit length, x2 ~ R x1 + t, in units of the baseline (the convention of
+ *                                dgb200_pose_from_fundamental_ragged_dev: candidate 0 goes straight into
+ *                                dgb200_refine_pose_ragged_dev);
+ *   d_plane_out [n_pairs][2][4]  (n, d): the plane n^T X = d in camera 1's frame, baseline units, d = 1/|t'| > 0;
+ *   d_good_out [n_pairs][2]      the votes;
+ *   d_rotation_only_out [n_pairs] 1 for a pure rotation.
+ * A pure rotation's candidate 0 has t = 0 and a NaN plane; its candidate 1 is R = t = 0, plane NaN, good 0.
+ * Per row r under candidate 0, the definitions of dgb200_pose_from_fundamental_ragged_dev: d_points_out (midpoint),
+ * d_in_front_out (mask && l1 > 0 && l2 > 0), d_angle_out (parallax), and d_median_angle_out per pair (exact median of
+ * the in-front rows' angles, NaN when there is none).  A pure rotation's rows get NaN points and
+ * in_front = mask && x1 . R^T x2 > 0; its angles and median are computed as usual (the median is the value that
+ * COLMAP-style code compares with a threshold to call a pair panoramic).  A pair whose H is all zero (no model) or
+ * holds a NaN gets R = t = 0 and NaN planes for both candidates, good 0, rotation_only 0, NaN points and angles,
+ * in_front 0 and a NaN median.  Offsets that decrease, are negative or pass `rows` make an empty pair: no row is read or
+ * written.  d_mask and d_good_out may be NULL; the row arrays may be NULL when rows = 0; every other buffer is required.
+ * A null required buffer, n_pairs < 1, rows < 0 or dim < 2 returns DGB200_E_ARG before any launch.  Asynchronous on
+ * `stream`, one kernel, no workspace; a pair's result does not depend on the batch it is in. */
+int dgb200_pose_from_homography_ragged_dev(const double* d_H, const double* d_K1, const double* d_K2, int k_per_pair,
+                                           const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets,
+                                           int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                           double* d_R_out, double* d_t_out, double* d_plane_out, int32_t* d_good_out,
+                                           uint8_t* d_rotation_only_out, double* d_points_out, uint8_t* d_in_front_out,
+                                           double* d_angle_out, double* d_median_angle_out, void* stream);
 /* Refinement of the relative pose on the inliers, over a RAGGED batch laid out as above (d_offsets, d_x1y1 / d_x2y2,
  * d_mask, K): per pair, Levenberg-Marquardt from (d_R [n_pairs][9] row-major, d_t [n_pairs][3] of unit length; what
  * dgb200_pose_from_fundamental_ragged_dev returns) on the cost C(R, t) = sum of r^2 over the rows with mask != 0, r the

@@ -66,6 +66,8 @@ def lib():
         L.dgb200_pose_from_fundamental_batch_dev.argtypes =[vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
         L.dgb200_pose_from_fundamental_ragged_dev.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp, vp, vp,
                                                               vp, vp, vp]
+        L.dgb200_pose_from_homography_ragged_dev.argtypes = [vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, vp, vp, vp, vp,
+                                                             vp, vp, vp, vp, vp, vp]
         L.dgb200_refine_pose_ragged_dev.argtypes = [vp, vp, vp, vp, ci, vp, vp, vp, ci, ci, ci, vp, ci, cd, vp, vp, vp, vp,
                                                     vp, vp, vp, vp, vp]
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]

@@ -10,6 +10,8 @@
 //           (cp.async.bulk global->shared, completion on an mbarrier; UBLKCP in SASS), double buffered behind the math.
 //   AFTER   pose from a fundamental matrix: E = K2^T F K1, the four (R, t) candidates, cheirality vote over the
 //           inliers (one warp per pair);  the reference stops at F (the survey lists E/pose as the step after).
+//           Pose and scene plane from a homography (planar scenes, pure rotations): the decompositions of
+//           K2^-1 H K1, cheirality vote, the two best candidates; the rows and median of the F path.
 //   ALSO    the reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594, USE_QR) as a batch
 //           kernel over many samples (la.h restates LAPACK's dgeqp3 kernel).
 #include <cuda_runtime.h>
@@ -610,17 +612,30 @@ __global__ void pose_kernel(PoseArgs a) {
   }
 }
 
-// ------------------------------------------------------------------------------------------------ pose from F, ragged
+// ------------------------------------------------------------------------------------------------ pose, ragged
 constexpr int kPoseThreads = 256;     // = the 256 bins of the median's radix select: one bin per thread
 
-struct PoseRaggedArgs {
-  const double* F; const double* K1; const double* K2;   // [P][9] row-major; K: [9] shared or [P][9]
+// The ragged layout and the per-row outputs that the two ragged pose kernels (from F, from H) share.
+struct PoseRows {
+  const double* K1; const double* K2;                      // K: [9] shared or [P][9], row-major
   int k_per_pair;
   const double* x1y1; const double* x2y2; const int* offsets; const unsigned char* mask;   // [rows][dim], [P+1], [rows]
   int n_pairs, rows, dim;
-  double* R; double* t; int* good;                        // [P][9], [P][3], [P] (or null)
   double* points; unsigned char* in_front; double* angle;   // [rows][3], [rows], [rows]
   double* median;                                         // [P]
+};
+
+struct PoseRaggedArgs {
+  PoseRows w;
+  const double* F;                                        // [P][9] row-major
+  double* R; double* t; int* good;                        // [P][9], [P][3], [P] (or null)
+};
+
+struct PoseHRaggedArgs {
+  PoseRows w;
+  const double* H;                                        // [P][9] row-major, x2 ~ H x1
+  double* R; double* t; double* plane; int* good;         // [P][2][9], [P][2][3], [P][2][4], [P][2] (or null)
+  unsigned char* rotation_only;                           // [P]
 };
 
 // Exclusive prefix of v over the CTA's threads (in thread order) and the CTA's total; ws: kPoseThreads / 32 ints.
@@ -641,115 +656,115 @@ __device__ __forceinline__ int pose_block_scan(int v, int* ws, int* total) {
   return off + x - v;
 }
 
-// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1.
-//   pass 1: lane 0 of warp 0 builds the four candidates (pose_candidates), lane 1 the inverse calibrations;
-//   pass 2: the block votes over the rows with mask != 0 (pose_depths), first candidate wins ties -- the arithmetic and
-//           tie rule of pose_kernel, so R, t, good are those of a dense call on the pair alone;
-//   pass 3: per row under the chosen (R, t): in_front = mask && l1 > 0 && l2 > 0, the midpoint
-//           0.5 (l1 x1 + R^T (l2 x2 - t)) in camera 1's frame, the parallax angle atan2(|x1 x R^T x2|, x1 . R^T x2);
-//   pass 4: the median of the angles of the in-front rows, read back from global memory after a barrier: a radix
-//           select over the bit patterns of the (non-negative) doubles, eight 8-bit digits from the top, which needs no
-//           workspace and no bound on the row count.  An even count averages the two middle values as np.median does.
-// A pair whose F is all zero (no model) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, in_front = 0,
-// median NaN.  Offsets that decrease, are negative or pass `rows` make an empty pair: no row is read or written.
-__global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArgs a) {
-  __shared__ double cand[4 * 12];
-  __shared__ double kinv[18];
-  __shared__ int ws[kPoseThreads / 32];
-  __shared__ int wvotes[kPoseThreads / 32][4];
-  __shared__ unsigned hist[256];
-  __shared__ int s_best, s_digit, s_below, s_eq;
-  __shared__ unsigned long long s_min[kPoseThreads / 32];
-  const int p = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const int b = a.offsets[p], e = a.offsets[p + 1];
-  const bool span_ok = b >= 0 && b <= e && e <= a.rows;
-  const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
-  const double* F = a.F + (size_t)p * 9;
-  bool zero = true, has_nan = false;
-  for (int i = 0; i < 9; ++i) { zero &= F[i] == 0.0; has_nan |= F[i] != F[i]; }
-  if (zero || has_nan) {                          // (block-uniform)
-    for (int i = tid; i < n; i += kPoseThreads) {
-      const size_t r = (size_t)r0 + i;
-      for (int c = 0; c < 3; ++c) a.points[3 * r + c] = qnan();
-      a.in_front[r] = 0;
-      a.angle[r] = qnan();
-    }
-    if (tid < 9) a.R[(size_t)p * 9 + tid] = 0.0;
-    if (tid < 3) a.t[(size_t)p * 3 + tid] = 0.0;
-    if (tid == 0) {
-      if (a.good) a.good[p] = 0;
-      a.median[p] = qnan();
-    }
-    return;
-  }
-  const double* K1 = a.K1 + (a.k_per_pair ? (size_t)p * 9 : 0);
-  const double* K2 = a.K2 + (a.k_per_pair ? (size_t)p * 9 : 0);
-  if (tid == 0) pose_candidates(F, K1, K2, cand);
-  if (tid == 1) {                                 // the inverse calibrations (dg::inv3, as pose_kernel)
-    for (int i = 0; i < 9; ++i) { kinv[i] = K1[i]; kinv[9 + i] = K2[i]; }
-    dg::inv3(kinv);
-    dg::inv3(kinv + 9);
-  }
-  __syncthreads();
+// Pair p's rows r0 .. r0 + n - 1; offsets that decrease, are negative or pass `rows` make an empty pair.
+__device__ __forceinline__ void pose_span(const PoseRows& w, int p, int* r0, int* n) {
+  const int b = w.offsets[p], e = w.offsets[p + 1];
+  const bool span_ok = b >= 0 && b <= e && e <= w.rows;
+  *r0 = span_ok ? b : 0;
+  *n = span_ok ? e - b : 0;
+}
 
-  const unsigned char* mk = a.mask;
-  const double* g1 = a.x1y1;
-  const double* g2 = a.x2y2;
-  const int dim = a.dim;
-  int votes[4] = {0, 0, 0, 0};
+// The rows of a pair without a model: NaN points and angles, in_front = 0.
+__device__ __forceinline__ void pose_rows_void(const PoseRows& w, int r0, int n) {
+  for (int i = threadIdx.x; i < n; i += kPoseThreads) {
+    const size_t r = (size_t)r0 + i;
+    for (int c = 0; c < 3; ++c) w.points[3 * r + c] = qnan();
+    w.in_front[r] = 0;
+    w.angle[r] = qnan();
+  }
+}
+
+// The inverse calibrations K1^-1, K2^-1 of pair p into kinv[18] (dg::inv3, as pose_kernel).
+__device__ __forceinline__ void pose_kinv(const PoseRows& w, int p, double* kinv) {
+  const double* K1 = w.K1 + (w.k_per_pair ? (size_t)p * 9 : 0);
+  const double* K2 = w.K2 + (w.k_per_pair ? (size_t)p * 9 : 0);
+  for (int i = 0; i < 9; ++i) { kinv[i] = K1[i]; kinv[9 + i] = K2[i]; }
+  dg::inv3(kinv);
+  dg::inv3(kinv + 9);
+}
+
+// y = R^T x.
+__device__ __forceinline__ void pose_back_rotate(const double* R, const double* x, double* y) {
+  for (int c = 0; c < 3; ++c) y[c] = R[c] * x[0] + R[3 + c] * x[1] + R[6 + c] * x[2];
+}
+
+// The block's vote: per candidate c < NC, the rows with mask != 0 whose rays x1, x2 `supports(c, x1, x2)` accepts.
+// Counted per thread, reduced per warp by shuffles and over the warps in a fixed order; the totals tot[NC] are valid
+// in thread 0.  Called by all threads; ends with a barrier.
+template <int NC, class Supports>
+__device__ __forceinline__ void pose_vote(const PoseRows& w, int r0, int n, const double* kinv, Supports supports,
+                                          int (*wvotes)[NC], int* tot) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const unsigned char* mk = w.mask;
+  const double* g1 = w.x1y1;
+  const double* g2 = w.x2y2;
+  const int dim = w.dim;
+  int votes[NC];
+  for (int c = 0; c < NC; ++c) votes[c] = 0;
   for (int i = tid; i < n; i += kPoseThreads) {
     const size_t r = (size_t)r0 + i;
     if (mk && !mk[r]) continue;
     double x1[3], x2[3];
     pose_ray(kinv, g1[r * dim], g1[r * dim + 1], x1);
     pose_ray(kinv + 9, g2[r * dim], g2[r * dim + 1], x2);
-    for (int c = 0; c < 4; ++c) {
-      double l1, l2;
-      pose_depths(cand + 12 * c, cand + 12 * c + 9, x1, x2, &l1, &l2);
-      if (l1 > 0 && l2 > 0) ++votes[c];
-    }
+    for (int c = 0; c < NC; ++c)
+      if (supports(c, x1, x2)) ++votes[c];
   }
-  for (int c = 0; c < 4; ++c)
+  for (int c = 0; c < NC; ++c)
     for (int o = 16; o > 0; o >>= 1) votes[c] += __shfl_xor_sync(0xffffffffu, votes[c], o);
-  if (lane == 0) for (int c = 0; c < 4; ++c) wvotes[wid][c] = votes[c];
+  if (lane == 0) for (int c = 0; c < NC; ++c) wvotes[wid][c] = votes[c];
   __syncthreads();
   if (tid == 0) {
-    int tot[4] = {0, 0, 0, 0};
-    for (int w = 0; w < kPoseThreads / 32; ++w) for (int c = 0; c < 4; ++c) tot[c] += wvotes[w][c];
-    int best = 0;
-    for (int c = 1; c < 4; ++c) if (tot[c] > tot[best]) best = c;
-    s_best = best;
-    wvotes[0][0] = tot[best];
-    if (a.good) a.good[p] = tot[best];
+    for (int c = 0; c < NC; ++c) tot[c] = 0;
+    for (int v = 0; v < kPoseThreads / 32; ++v) for (int c = 0; c < NC; ++c) tot[c] += wvotes[v][c];
   }
-  __syncthreads();
-  const int best = s_best, count = wvotes[0][0];
-  const double* Rb = cand + 12 * best;
-  const double* tb = Rb + 9;
-  if (tid < 9) a.R[(size_t)p * 9 + tid] = Rb[tid];
-  if (tid < 3) a.t[(size_t)p * 3 + tid] = tb[tid];
+}
 
-  for (int i = tid; i < n; i += kPoseThreads) {
+// Per row under the pose (R, t): the parallax angle atan2(|x1 x R^T x2|, x1 . R^T x2) and
+//   translation (rotation = false): in_front = mask && l1 > 0 && l2 > 0 with (l1, l2) of pose_depths, the midpoint
+//     0.5 (l1 x1 + R^T (l2 x2 - t)) in camera 1's frame;
+//   pure rotation (rotation = true, t unused): in_front = mask && x1 . R^T x2 > 0, NaN points (no depth).
+__device__ __forceinline__ void pose_rows_under(const PoseRows& w, int r0, int n, const double* kinv, const double* Rb,
+                                                const double* tb, bool rotation) {
+  const unsigned char* mk = w.mask;
+  const double* g1 = w.x1y1;
+  const double* g2 = w.x2y2;
+  const int dim = w.dim;
+  for (int i = threadIdx.x; i < n; i += kPoseThreads) {
     const size_t r = (size_t)r0 + i;
-    double x1[3], x2[3], l1, l2;
+    double x1[3], x2[3], y[3];                     // y = R^T x2
     pose_ray(kinv, g1[r * dim], g1[r * dim + 1], x1);
     pose_ray(kinv + 9, g2[r * dim], g2[r * dim + 1], x2);
-    pose_depths(Rb, tb, x1, x2, &l1, &l2);
-    a.in_front[r] = (!mk || mk[r]) && l1 > 0 && l2 > 0;
-    double y[3], q[3];                             // y = R^T x2, q = l2 x2 - t
-    for (int c = 0; c < 3; ++c) {
-      y[c] = Rb[c] * x2[0] + Rb[3 + c] * x2[1] + Rb[6 + c] * x2[2];
-      q[c] = l2 * x2[c] - tb[c];
+    if (rotation) {
+      pose_back_rotate(Rb, x2, y);
+      w.in_front[r] = (!mk || mk[r]) && x1[0] * y[0] + x1[1] * y[1] + x1[2] * y[2] > 0;
+      for (int c = 0; c < 3; ++c) w.points[3 * r + c] = qnan();
+    } else {
+      double l1, l2, q[3];                         // q = l2 x2 - t
+      pose_depths(Rb, tb, x1, x2, &l1, &l2);
+      w.in_front[r] = (!mk || mk[r]) && l1 > 0 && l2 > 0;
+      for (int c = 0; c < 3; ++c) {
+        y[c] = Rb[c] * x2[0] + Rb[3 + c] * x2[1] + Rb[6 + c] * x2[2];
+        q[c] = l2 * x2[c] - tb[c];
+      }
+      for (int c = 0; c < 3; ++c)
+        w.points[3 * r + c] = 0.5 * (l1 * x1[c] + (Rb[c] * q[0] + Rb[3 + c] * q[1] + Rb[6 + c] * q[2]));
     }
-    for (int c = 0; c < 3; ++c)
-      a.points[3 * r + c] = 0.5 * (l1 * x1[c] + (Rb[c] * q[0] + Rb[3 + c] * q[1] + Rb[6 + c] * q[2]));
     const double cx = x1[1] * y[2] - x1[2] * y[1], cy = x1[2] * y[0] - x1[0] * y[2], cz = x1[0] * y[1] - x1[1] * y[0];
-    a.angle[r] = atan2(sqrt(cx * cx + cy * cy + cz * cz), x1[0] * y[0] + x1[1] * y[1] + x1[2] * y[2]);
+    w.angle[r] = atan2(sqrt(cx * cx + cy * cy + cz * cz), x1[0] * y[0] + x1[1] * y[1] + x1[2] * y[2]);
   }
-  if (count == 0) {                                // (block-uniform)
-    if (tid == 0) a.median[p] = qnan();
-    return;
-  }
+}
+
+// The median of the angles of the pair's in-front rows, count > 0 of them, read back from global memory after a
+// barrier: a radix select over the bit patterns of the (non-negative) doubles, eight 8-bit digits from the top, which
+// needs no workspace and no bound on the row count.  An even count averages the two middle values as np.median does.
+// Called by all threads after the row pass; the result is valid in thread 0.
+__device__ __forceinline__ double pose_median(const PoseRows& w, int r0, int n, int count) {
+  __shared__ int ws[kPoseThreads / 32];
+  __shared__ unsigned hist[256];
+  __shared__ int s_digit, s_below, s_eq;
+  __shared__ unsigned long long s_min[kPoseThreads / 32];
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   __syncthreads();                                 // this CTA's angle / in_front rows are visible to all its threads
 
   // k-th smallest key (k = (count - 1) / 2) among the in-front rows: fix 8 bits per pass, from the top
@@ -760,8 +775,8 @@ __global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArg
     __syncthreads();
     for (int i = tid; i < n; i += kPoseThreads) {
       const size_t r = (size_t)r0 + i;
-      if (!a.in_front[r]) continue;
-      const unsigned long long key = (unsigned long long)__double_as_longlong(a.angle[r]);
+      if (!w.in_front[r]) continue;
+      const unsigned long long key = (unsigned long long)__double_as_longlong(w.angle[r]);
       if ((key & known) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
     }
     __syncthreads();
@@ -775,18 +790,15 @@ __global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArg
     known |= 255ull << shift;
   }
   const double lo = __longlong_as_double((long long)prefix);
-  if (count & 1) {
-    if (tid == 0) a.median[p] = lo;
-    return;
-  }
+  if (count & 1) return lo;
   // even count: the next order statistic is lo again when lo has further copies, else the smallest key above it
   double hi = lo;
   if (k + 1 >= s_eq) {                             // (block-uniform)
     unsigned long long m = ~0ull;
     for (int i = tid; i < n; i += kPoseThreads) {
       const size_t r = (size_t)r0 + i;
-      if (!a.in_front[r]) continue;
-      const unsigned long long key = (unsigned long long)__double_as_longlong(a.angle[r]);
+      if (!w.in_front[r]) continue;
+      const unsigned long long key = (unsigned long long)__double_as_longlong(w.angle[r]);
       if (key > prefix && key < m) m = key;
     }
     for (int o = 16; o > 0; o >>= 1) {
@@ -796,11 +808,250 @@ __global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArg
     if (lane == 0) s_min[wid] = m;
     __syncthreads();
     if (tid == 0) {
-      for (int w = 1; w < kPoseThreads / 32; ++w) m = s_min[w] < m ? s_min[w] : m;
+      for (int v = 1; v < kPoseThreads / 32; ++v) m = s_min[v] < m ? s_min[v] : m;
       hi = __longlong_as_double((long long)m);
     }
   }
-  if (tid == 0) a.median[p] = (lo + hi) / 2.0;
+  return (lo + hi) / 2.0;
+}
+
+// The rows and the median of a pair under its chosen pose (pose_rows_under, then pose_median); count = the pair's
+// in-front rows, known from the vote.  Called by all threads.
+__device__ __forceinline__ void pose_rows_and_median(const PoseRows& w, int p, int r0, int n, const double* kinv,
+                                                     const double* Rb, const double* tb, bool rotation, int count) {
+  pose_rows_under(w, r0, n, kinv, Rb, tb, rotation);
+  if (count == 0) {                                // (block-uniform)
+    if (threadIdx.x == 0) w.median[p] = qnan();
+    return;
+  }
+  const double med = pose_median(w, r0, n, count);
+  if (threadIdx.x == 0) w.median[p] = med;
+}
+
+// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1.
+//   pass 1: thread 0 builds the four candidates (pose_candidates), thread 1 the inverse calibrations;
+//   pass 2: the block votes over the rows with mask != 0 (pose_depths), first candidate wins ties -- the arithmetic and
+//           tie rule of pose_kernel, so R, t, good are those of a dense call on the pair alone;
+//   pass 3: per row under the chosen (R, t) (pose_rows_under);
+//   pass 4: the median of the angles of the in-front rows (pose_median).
+// A pair whose F is all zero (no model) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, in_front = 0,
+// median NaN.  Offsets that decrease, are negative or pass `rows` make an empty pair: no row is read or written.
+__global__ void __launch_bounds__(kPoseThreads) pose_ragged_kernel(PoseRaggedArgs a) {
+  __shared__ double cand[4 * 12];
+  __shared__ double kinv[18];
+  __shared__ int wvotes[kPoseThreads / 32][4];
+  __shared__ int s_best;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  int r0, n;
+  pose_span(a.w, p, &r0, &n);
+  const double* F = a.F + (size_t)p * 9;
+  bool zero = true, has_nan = false;
+  for (int i = 0; i < 9; ++i) { zero &= F[i] == 0.0; has_nan |= F[i] != F[i]; }
+  if (zero || has_nan) {                          // (block-uniform)
+    pose_rows_void(a.w, r0, n);
+    if (tid < 9) a.R[(size_t)p * 9 + tid] = 0.0;
+    if (tid < 3) a.t[(size_t)p * 3 + tid] = 0.0;
+    if (tid == 0) {
+      if (a.good) a.good[p] = 0;
+      a.w.median[p] = qnan();
+    }
+    return;
+  }
+  if (tid == 0)
+    pose_candidates(F, a.w.K1 + (a.w.k_per_pair ? (size_t)p * 9 : 0), a.w.K2 + (a.w.k_per_pair ? (size_t)p * 9 : 0),
+                    cand);
+  if (tid == 1) pose_kinv(a.w, p, kinv);
+  __syncthreads();
+
+  int tot[4];
+  pose_vote<4>(a.w, r0, n, kinv, [&](int c, const double* x1, const double* x2) {
+    double l1, l2;
+    pose_depths(cand + 12 * c, cand + 12 * c + 9, x1, x2, &l1, &l2);
+    return l1 > 0 && l2 > 0;
+  }, wvotes, tot);
+  if (tid == 0) {
+    int best = 0;
+    for (int c = 1; c < 4; ++c) if (tot[c] > tot[best]) best = c;
+    s_best = best;
+    wvotes[0][0] = tot[best];
+    if (a.good) a.good[p] = tot[best];
+  }
+  __syncthreads();
+  const int best = s_best, count = wvotes[0][0];
+  const double* Rb = cand + 12 * best;
+  const double* tb = Rb + 9;
+  if (tid < 9) a.R[(size_t)p * 9 + tid] = Rb[tid];
+  if (tid < 3) a.t[(size_t)p * 3 + tid] = tb[tid];
+  pose_rows_and_median(a.w, p, r0, n, kinv, Rb, tb, false, count);
+}
+
+// ------------------------------------------------------------------------------------------------ pose from H, ragged
+constexpr double kRotationTol = 1e-3;   // max |Hn^T Hn - I| below which Hn is taken for a rotation (cv2's rule)
+
+// Candidates of pose from a homography, FP64 on one thread, into cand[4][16] = (R row-major [9], t [3], n [3], d).
+// Hn = K2^-1 H K1 divided by its middle singular value (dg::svd3_onesided) and negated when det(Hn) < 0.
+//   max |S_ij| < kRotationTol with S = Hn^T Hn - I: a pure rotation, ONE candidate: R = U V^T (the rotation nearest to
+//     Hn), t = 0, n = d = NaN.  Returns 1.
+//   otherwise the four decompositions Hn = R + t' n^T, |n| = 1, of Malis & Vargas (INRIA RR-6303, 2007, section 4, the
+//     analytical method) in the order (Ra, t'a, na), (Ra, -t'a, -na), (Rb, t'b, nb), (Rb, -t'b, -nb) -- the order of
+//     cv2.decomposeHomographyMat -- stored as t = t' / |t'| and the plane n^T X = d, d = 1 / |t'|.  Returns 4.
+__device__ int pose_h_candidates(const double* H, const double* K1, const double* K2, double* cand) {
+  double Hn[9];
+  {
+    double K2i[9], T[9];
+    for (int i = 0; i < 9; ++i) K2i[i] = K2[i];
+    dg::inv3(K2i);
+    mat3_mul(K2i, H, T);
+    mat3_mul(T, K1, Hn);
+  }
+  double G[9], V[9], sv[3];
+  dg::svd3_onesided(Hn, G, V, sv);
+  const double mid = fmax(fmin(sv[0], sv[1]), fmin(fmax(sv[0], sv[1]), sv[2]));
+  for (int i = 0; i < 9; ++i) Hn[i] /= mid;
+  if (det3r(Hn) < 0) for (int i = 0; i < 9; ++i) Hn[i] = -Hn[i];
+  double S[9], smax = 0.0;
+  for (int i = 0; i < 3; ++i)
+    for (int j = 0; j < 3; ++j) {
+      S[3 * i + j] = Hn[i] * Hn[j] + Hn[3 + i] * Hn[3 + j] + Hn[6 + i] * Hn[6 + j] - (i == j ? 1.0 : 0.0);
+      smax = fmax(smax, fabs(S[3 * i + j]));
+    }
+  if (smax < kRotationTol) {
+    dg::svd3_onesided(Hn, G, V, sv);               // Hn = U diag(sv) V^T, U = G diag(1 / sv)
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j)
+        cand[3 * i + j] = G[3 * i] / sv[0] * V[3 * j] + G[3 * i + 1] / sv[1] * V[3 * j + 1] +
+                          G[3 * i + 2] / sv[2] * V[3 * j + 2];
+    for (int i = 9; i < 12; ++i) cand[i] = 0.0;
+    for (int i = 12; i < 16; ++i) cand[i] = qnan();
+    return 1;
+  }
+  // opposites of the principal minors of S (>= 0), and of the off-diagonal ones (their signs pick the roots)
+  const double s11 = S[0], s12 = S[1], s13 = S[2], s22 = S[4], s23 = S[5], s33 = S[8];
+  const double m11 = s23 * s23 - s22 * s33, m22 = s13 * s13 - s11 * s33, m33 = s12 * s12 - s11 * s22;
+  const double m12 = s23 * s13 - s12 * s33, m13 = s22 * s13 - s12 * s23, m23 = s12 * s13 - s11 * s23;
+  const double r11 = sqrt(fmax(m11, 0.0)), r22 = sqrt(fmax(m22, 0.0)), r33 = sqrt(fmax(m33, 0.0));
+  const double d1 = fabs(s11), d2 = fabs(s22), d3 = fabs(s33);
+  const int ii = (d1 >= d2 && d1 >= d3) ? 0 : (d2 >= d3 ? 1 : 2);   // the largest |s_ii| keeps n' away from zero
+  double na[3], nb[3], es;
+  if (ii == 0) {
+    const double e = m23 >= 0 ? 1.0 : -1.0;
+    na[0] = s11; na[1] = s12 + r33; na[2] = s13 + e * r22;
+    nb[0] = s11; nb[1] = s12 - r33; nb[2] = s13 - e * r22;
+    es = s11 >= 0 ? 1.0 : -1.0;
+  } else if (ii == 1) {
+    const double e = m13 >= 0 ? 1.0 : -1.0;
+    na[0] = s12 + r33; na[1] = s22; na[2] = s23 - e * r11;
+    nb[0] = s12 - r33; nb[1] = s22; nb[2] = s23 + e * r11;
+    es = s22 >= 0 ? 1.0 : -1.0;
+  } else {
+    const double e = m12 >= 0 ? 1.0 : -1.0;
+    na[0] = s13 + e * r22; na[1] = s23 + r11; na[2] = s33;
+    nb[0] = s13 - e * r22; nb[1] = s23 - r11; nb[2] = s33;
+    es = s33 >= 0 ? 1.0 : -1.0;
+  }
+  const double la = sqrt(na[0] * na[0] + na[1] * na[1] + na[2] * na[2]);
+  const double lb = sqrt(nb[0] * nb[0] + nb[1] * nb[1] + nb[2] * nb[2]);
+  for (int i = 0; i < 3; ++i) { na[i] /= la; nb[i] /= lb; }
+  const double tr = s11 + s22 + s33;
+  const double nu = 2.0 * sqrt(fmax(1.0 + tr - m11 - m22 - m33, 0.0));
+  const double rho = sqrt(2.0 + tr + nu);
+  const double te = sqrt(fmax(2.0 + tr - nu, 0.0));
+  for (int s = 0; s < 2; ++s) {                    // s = 0: (Ra, t'a, na), s = 1: (Rb, t'b, nb)
+    const double* n1 = s ? nb : na;
+    const double* n2 = s ? na : nb;
+    double ts[3], R[9], t[3];                      // ts = R^T t': t' in camera 1's frame
+    for (int i = 0; i < 3; ++i) ts[i] = 0.5 * te * (es * rho * n2[i] - te * n1[i]);
+    {
+      double M[9];                                 // R = Hn (I - (2 / nu) ts n^T)
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) M[3 * i + j] = (i == j ? 1.0 : 0.0) - (2.0 / nu) * ts[i] * n1[j];
+      mat3_mul(Hn, M, R);
+    }
+    for (int i = 0; i < 3; ++i) t[i] = R[3 * i] * ts[0] + R[3 * i + 1] * ts[1] + R[3 * i + 2] * ts[2];
+    const double tn = sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
+    for (int c = 0; c < 2; ++c) {                  // c = 1: (R, -t', -n)
+      double* o = cand + 16 * (2 * s + c);
+      const double sg = c ? -1.0 : 1.0;
+      for (int i = 0; i < 9; ++i) o[i] = R[i];
+      for (int i = 0; i < 3; ++i) { o[9 + i] = sg * t[i] / tn; o[12 + i] = sg * n1[i]; }
+      o[15] = 1.0 / tn;
+    }
+  }
+  return 4;
+}
+
+// One CTA per pair p over the ragged layout of pose_ragged_kernel.
+//   pass 1: thread 0 builds the candidates (pose_h_candidates), thread 1 the inverse calibrations;
+//   pass 2: the block votes over the rows with mask != 0: a candidate (R, t) is supported by a row when pose_depths
+//           gives both depths positive; the rotation by a row with x1 . R^T x2 > 0.  Candidate 0 is the one with the
+//           most votes, candidate 1 the one with the most among the rest, ties to the earlier candidate;
+//   passes 3, 4: the rows under candidate 0 and the median, as pose_ragged_kernel (pose_rows_and_median).
+// A rotation-only pair's candidate 1 is R = t = 0, plane NaN, good 0.  A pair whose H is all zero (no model) or holds a
+// NaN gets R = t = 0 and plane NaN for both candidates, good 0, NaN points and angles, in_front = 0, median NaN.  Offsets
+// that decrease, are negative or pass `rows` make an empty pair: no row is read or written.
+__global__ void __launch_bounds__(kPoseThreads) pose_h_ragged_kernel(PoseHRaggedArgs a) {
+  __shared__ double cand[4 * 16];
+  __shared__ double kinv[18];
+  __shared__ int wvotes[kPoseThreads / 32][4];
+  __shared__ int s_nc, s_first, s_count;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  int r0, n;
+  pose_span(a.w, p, &r0, &n);
+  const double* H = a.H + (size_t)p * 9;
+  bool zero = true, has_nan = false;
+  for (int i = 0; i < 9; ++i) { zero &= H[i] == 0.0; has_nan |= H[i] != H[i]; }
+  if (zero || has_nan) {                          // (block-uniform)
+    pose_rows_void(a.w, r0, n);
+    if (tid < 18) a.R[(size_t)p * 18 + tid] = 0.0;
+    if (tid < 6) a.t[(size_t)p * 6 + tid] = 0.0;
+    if (tid < 8) a.plane[(size_t)p * 8 + tid] = qnan();
+    if (tid < 2 && a.good) a.good[(size_t)p * 2 + tid] = 0;
+    if (tid == 0) {
+      a.rotation_only[p] = 0;
+      a.w.median[p] = qnan();
+    }
+    return;
+  }
+  if (tid == 0)
+    s_nc = pose_h_candidates(H, a.w.K1 + (a.w.k_per_pair ? (size_t)p * 9 : 0),
+                             a.w.K2 + (a.w.k_per_pair ? (size_t)p * 9 : 0), cand);
+  if (tid == 1) pose_kinv(a.w, p, kinv);
+  __syncthreads();
+
+  const int nc = s_nc;
+  const bool rotation = nc == 1;
+  int tot[4];
+  pose_vote<4>(a.w, r0, n, kinv, [&](int c, const double* x1, const double* x2) {
+    if (c >= nc) return false;
+    const double* Rc = cand + 16 * c;
+    if (rotation) {
+      double y[3];
+      pose_back_rotate(Rc, x2, y);
+      return x1[0] * y[0] + x1[1] * y[1] + x1[2] * y[2] > 0;
+    }
+    double l1, l2;
+    pose_depths(Rc, Rc + 9, x1, x2, &l1, &l2);
+    return l1 > 0 && l2 > 0;
+  }, wvotes, tot);
+  if (tid == 0) {
+    int first = 0, second = -1;
+    for (int c = 1; c < nc; ++c) if (tot[c] > tot[first]) first = c;
+    for (int c = 0; c < nc; ++c) if (c != first && (second < 0 || tot[c] > tot[second])) second = c;
+    for (int slot = 0; slot < 2; ++slot) {
+      const int c = slot ? second : first;
+      const double* o = cand + 16 * (c < 0 ? 0 : c);
+      for (int i = 0; i < 9; ++i) a.R[(size_t)p * 18 + 9 * slot + i] = c < 0 ? 0.0 : o[i];
+      for (int i = 0; i < 3; ++i) a.t[(size_t)p * 6 + 3 * slot + i] = c < 0 ? 0.0 : o[9 + i];
+      for (int i = 0; i < 4; ++i) a.plane[(size_t)p * 8 + 4 * slot + i] = c < 0 ? qnan() : o[12 + i];
+      if (a.good) a.good[(size_t)p * 2 + slot] = c < 0 ? 0 : tot[c];
+    }
+    a.rotation_only[p] = rotation;
+    s_first = first;
+    s_count = tot[first];
+  }
+  __syncthreads();
+  const double* Rb = cand + 16 * s_first;
+  pose_rows_and_median(a.w, p, r0, n, kinv, Rb, Rb + 9, rotation, s_count);
 }
 
 // ------------------------------------------------------------------------------------------------ pose refinement, ragged
@@ -1165,6 +1416,16 @@ int match_batch(const void* d_bank, const int32_t* img_offsets, int n_images, in
                    guided ? guide : kNoGuide, d_models, px_th * px_th);
 }
 
+PoseRows pose_rows_args(const double* K1, const double* K2, int k_per_pair, const double* x1y1, const double* x2y2,
+                        const int32_t* offsets, int n_pairs, int rows, int dim, const uint8_t* mask, double* points,
+                        uint8_t* in_front, double* angle, double* median) {
+  PoseRows w;
+  w.K1 = K1; w.K2 = K2; w.k_per_pair = k_per_pair; w.x1y1 = x1y1; w.x2y2 = x2y2; w.offsets = offsets; w.mask = mask;
+  w.n_pairs = n_pairs; w.rows = rows; w.dim = dim; w.points = points; w.in_front = in_front; w.angle = angle;
+  w.median = median;
+  return w;
+}
+
 }  // namespace
 
 extern "C" {
@@ -1277,11 +1538,32 @@ int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K
     return fail2(DGB200_E_ARG, "null row buffer");
   if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
   PoseRaggedArgs a;
-  a.F = d_F; a.K1 = d_K1; a.K2 = d_K2; a.k_per_pair = k_per_pair; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2;
-  a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs; a.rows = rows; a.dim = dim;
-  a.R = d_R_out; a.t = d_t_out; a.good = d_good_out; a.points = d_points_out; a.in_front = d_in_front_out;
-  a.angle = d_angle_out; a.median = d_median_angle_out;
+  a.w = pose_rows_args(d_K1, d_K2, k_per_pair, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask, d_points_out,
+                       d_in_front_out, d_angle_out, d_median_angle_out);
+  a.F = d_F; a.R = d_R_out; a.t = d_t_out; a.good = d_good_out;
   pose_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
+int dgb200_pose_from_homography_ragged_dev(const double* d_H, const double* d_K1, const double* d_K2, int k_per_pair,
+                                           const double* d_x1y1, const double* d_x2y2, const int32_t* d_offsets,
+                                           int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                           double* d_R_out, double* d_t_out, double* d_plane_out, int32_t* d_good_out,
+                                           uint8_t* d_rotation_only_out, double* d_points_out, uint8_t* d_in_front_out,
+                                           double* d_angle_out, double* d_median_angle_out, void* stream) {
+  if (!d_H || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_plane_out || !d_rotation_only_out ||
+      !d_median_angle_out)
+    return fail2(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x1y1 || !d_x2y2 || !d_points_out || !d_in_front_out || !d_angle_out))
+    return fail2(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  PoseHRaggedArgs a;
+  a.w = pose_rows_args(d_K1, d_K2, k_per_pair, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask, d_points_out,
+                       d_in_front_out, d_angle_out, d_median_angle_out);
+  a.H = d_H; a.R = d_R_out; a.t = d_t_out; a.plane = d_plane_out; a.good = d_good_out;
+  a.rotation_only = d_rotation_only_out;
+  pose_h_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
   CU2(cudaGetLastError());
   return 0;
 }

@@ -29,6 +29,11 @@ Relative pose, triangulated points and parallax angles of the ragged result, sti
 The pose refined on its inliers (Levenberg-Marquardt on the Sampson error), with the calibrated F for a guided re-match:
 
     fine = refine_pose_ragged(pose.R, pose.t, K1, K2, m.pts1, m.pts2, m.offsets, pose.in_front)
+
+The H branch (planar scenes, pure rotations): pose and scene plane from H, the best two of its decompositions:
+
+    H, hmask = pydegensac_b200.findHomographyBatch(m.pts1, m.pts2, 2.0, 0.999, 10000, offsets=m.offsets, n_max=m.n_max)
+    hpose = pose_from_homography_ragged(H, K1, K2, m.pts1, m.pts2, m.offsets, hmask)
 """
 import collections
 import ctypes
@@ -43,6 +48,8 @@ BatchLayout = collections.namedtuple("BatchLayout", "tile_prefix row_prefix col_
 BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offsets n_max")
 RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angle median_angle")
 RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used iters inliers")
+HomographyPose = collections.namedtuple("HomographyPose",
+                                        "R t plane good rotation_only points in_front angle median_angle")
 
 
 def batch_layout(counts, pairs):
@@ -194,6 +201,48 @@ def pose_from_fundamental(F, K1, K2, pts1, pts2, mask=None):
     return R, t, good
 
 
+def _ragged_pose_inputs(model, name, K1, K2, pts1, pts2, offsets, mask):
+    """Checks the inputs of a ragged pose call (a [P,3,3] or [P,9] model named `name`, K, rows, offsets, mask) and returns
+    them ready for the C ABI: (P, rows, dim, device, per_pair, model, K1, K2, pts1, pts2, offsets, mask or None)."""
+    import torch
+    named = ((name, model), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % nm)
+    if model.dim() not in (2, 3) or model.shape[0] < 1 or tuple(model.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("%s must be [P,3,3] or [P,9] with P >= 1, not %s" % (name, list(model.shape)))
+    P = int(model.shape[0])
+    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
+        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
+    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
+    for nm, K in (("K1", K1), ("K2", K2)):
+        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
+            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (nm, P, list(K.shape)))
+    if tuple(offsets.shape) != (P + 1,):
+        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
+    if offsets.dtype != torch.int32:
+        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
+    for nm, x in ((name, model), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (rows,):
+            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    dev = pts1.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("%s, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device" % name)
+    per_pair = K1.dim() == 3 or K2.dim() == 3
+    if per_pair:
+        K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    f64 = torch.float64
+    Mc, K1c, K2c = (x.to(f64).contiguous() for x in (model, K1, K2))
+    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    return P, rows, dim, dev, int(per_pair), Mc, K1c, K2c, p1, p2, offsets.contiguous(), m
+
+
 def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
     """pose_from_fundamental over a ragged batch, with the triangulated points and parallax angles of every row.
 
@@ -209,42 +258,9 @@ def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
     (no model found) or holds a NaN gets R = t = 0, good = 0, NaN points and angles, no in-front row and a NaN median.
     Returns RaggedPose(R, t, good, points, in_front, angle, median_angle); asynchronous, nothing is read back."""
     import torch
-    named = (("F", F), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
-    for name, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % name)
-    if F.dim() not in (2, 3) or F.shape[0] < 1 or tuple(F.shape[1:]) not in ((3, 3), (9,)):
-        raise ValueError("F must be [P,3,3] or [P,9] with P >= 1, not %s" % list(F.shape))
-    P = int(F.shape[0])
-    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
-        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
-    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
-    for name, K in (("K1", K1), ("K2", K2)):
-        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
-            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (name, P, list(K.shape)))
-    if tuple(offsets.shape) != (P + 1,):
-        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
-    if offsets.dtype != torch.int32:
-        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    for name, x in (("F", F), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (rows,):
-            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    dev = pts1.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("F, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device")
-    per_pair = K1.dim() == 3 or K2.dim() == 3
-    if per_pair:
-        K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    P, rows, dim, dev, per_pair, Fc, K1c, K2c, p1, p2, off, m = _ragged_pose_inputs(F, "F", K1, K2, pts1, pts2,
+                                                                                    offsets, mask)
     f64 = torch.float64
-    Fc, K1c, K2c = (x.to(f64).contiguous() for x in (F, K1, K2))
-    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
-    off = offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
     with torch.cuda.device(dev):
         R = torch.empty((P, 3, 3), dtype=f64, device=dev)
@@ -256,13 +272,63 @@ def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
         median = torch.empty(P, dtype=f64, device=dev)
         vp = ctypes.c_void_p
         rc = L.dgb200_pose_from_fundamental_ragged_dev(
-            vp(Fc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), int(per_pair), vp(p1.data_ptr()),
+            vp(Fc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), per_pair, vp(p1.data_ptr()),
             vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim, vp(m.data_ptr()) if m is not None else None,
             vp(R.data_ptr()), vp(t.data_ptr()), vp(good.data_ptr()), vp(points.data_ptr()), vp(in_front.data_ptr()),
             vp(angle.data_ptr()), vp(median.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return RaggedPose(R, t, good, points, in_front.view(torch.bool), angle, median)
+
+
+def pose_from_homography_ragged(H, K1, K2, pts1, pts2, offsets, mask=None):
+    """Relative pose and scene plane from homographies over a ragged batch: the H branch's counterpart of
+    pose_from_fundamental_ragged, for planar scenes (F undetermined) and pure rotations (no F).
+
+    The inputs are what the ragged pipeline produces (match_descriptors_batch, then findHomographyBatch with offsets=),
+    all CUDA tensors on one device: H [P,3,3] or [P,9] (x2 ~ H x1, OpenCV convention), K1 / K2 [3,3] or [P,3,3], pts1 /
+    pts2 [rows, 2|6], offsets int32 [P+1], mask [rows] bool / uint8 or None (every row); floating inputs are used in
+    float64.  Per pair, Hn = K2^-1 H K1 is scaled to a middle singular value of 1 and det > 0.  When
+    max |Hn^T Hn - I| < 1e-3 the pair is a pure rotation: one candidate, the rotation nearest to Hn, t = 0.  Otherwise
+    Hn = R + t' n^T has the four solutions of cv2.decomposeHomographyMat, in its order (Malis & Vargas).  The rows with
+    mask set vote (both depths positive; x1 . R^T x2 > 0 for a rotation): candidate 0 has the most votes, candidate 1
+    the most among the rest, ties to the earlier solution.  Two views of a plane often leave both with equal votes, so
+    candidate 1 is returned for callers with a prior (ground-plane normal, a third view).
+    Returns HomographyPose(R, t, plane, good, rotation_only, points, in_front, angle, median_angle):
+    R [P,2,3,3]; t [P,2,3] unit length, x2 ~ R x1 + t (candidate 0 goes straight into refine_pose_ragged);
+    plane [P,2,4] (n, d), the plane n^T X = d in camera 1's frame and baseline units, d > 0; good [P,2] int32 the votes;
+    rotation_only [P] bool.  Per row, under candidate 0 and as pose_from_fundamental_ragged defines them: points [rows,3],
+    in_front [rows] bool, angle [rows]; median_angle [P].  A pure rotation has t = 0 and a NaN plane in candidate 0,
+    R = t = 0, a NaN plane and good 0 in candidate 1, NaN points and in_front = mask and x1 . R^T x2 > 0; its
+    median_angle is what COLMAP-style code compares with a threshold to call a pair panoramic.  A pair whose H is all zero
+    (no model found) or holds a NaN gets zero R and t, NaN planes, good 0, NaN rows and a NaN median.  Asynchronous,
+    nothing is read back."""
+    import torch
+    P, rows, dim, dev, per_pair, Hc, K1c, K2c, p1, p2, off, m = _ragged_pose_inputs(H, "H", K1, K2, pts1, pts2,
+                                                                                    offsets, mask)
+    f64 = torch.float64
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        R = torch.empty((P, 2, 3, 3), dtype=f64, device=dev)
+        t = torch.empty((P, 2, 3), dtype=f64, device=dev)
+        plane = torch.empty((P, 2, 4), dtype=f64, device=dev)
+        good = torch.empty((P, 2), dtype=torch.int32, device=dev)
+        rotation_only = torch.empty(P, dtype=torch.uint8, device=dev)
+        points = torch.empty((rows, 3), dtype=f64, device=dev)
+        in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
+        angle = torch.empty(rows, dtype=f64, device=dev)
+        median = torch.empty(P, dtype=f64, device=dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_pose_from_homography_ragged_dev(
+            vp(Hc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), per_pair, vp(p1.data_ptr()),
+            vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim, vp(m.data_ptr()) if m is not None else None,
+            vp(R.data_ptr()), vp(t.data_ptr()), vp(plane.data_ptr()), vp(good.data_ptr()), vp(rotation_only.data_ptr()),
+            vp(points.data_ptr()), vp(in_front.data_ptr()), vp(angle.data_ptr()), vp(median.data_ptr()),
+            vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_frontend_last_error().decode())
+    return HomographyPose(R, t, plane, good, rotation_only.view(torch.bool), points, in_front.view(torch.bool), angle,
+                          median)
 
 
 def refine_pose_ragged(R, t, K1, K2, pts1, pts2, offsets, mask=None, max_iters=10, px_th=None):
