@@ -23,7 +23,8 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
 from pydegensac_b200.matching import (match_descriptors, match_descriptors_guided, pose_from_fundamental,
-                                      pose_from_fundamental_ragged, pose_from_homography_ragged, refine_pose_ragged)
+                                      pose_from_fundamental_ragged, pose_from_homography_ragged,
+                                      refine_homography_ragged, refine_pose_ragged)
 from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
@@ -76,7 +77,11 @@ def main():
     q1, q2 = (torch.from_numpy(a).to(dev) for a in synth_plane())
     qoff = torch.tensor([0, len(q1)], dtype=torch.int32, device=dev)
     H, hmask = pydegensac.findHomographyBatch(q1, q2, 2.0, 0.999, 10000, seeds=[0], offsets=qoff, n_max=len(q1))
-    hp = pose_from_homography_ragged(H, K, K, q1, q2, qoff, hmask)
+    # H refined on its inliers (Sampson error of the RANSAC's rule), then pose from the refined H
+    fh = refine_homography_ragged(H, q1, q2, qoff, hmask, px_th=2.0)
+    print("H refined on %d rows in %d trial steps: summed Sampson error %.3f -> %.3f px^2, %d inliers at 2 px"
+          % (int(fh.n_used[0]), int(fh.iters[0]), float(fh.cost0[0]), float(fh.cost[0]), int(fh.inliers.sum())))
+    hp = pose_from_homography_ragged(fh.H, K, K, q1, q2, qoff, fh.inliers)
     for c, name in enumerate(("chosen", "runner-up")):
         print("H branch, %s pose (%d votes): R =\n" % (name, int(hp.good[0, c])), hp.R[0, c].cpu().numpy(),
               "\nt =", hp.t[0, c].cpu().numpy(), " plane n =", hp.plane[0, c, :3].cpu().numpy(),

@@ -336,6 +336,39 @@ int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const do
                                   double* d_R_out, double* d_t_out, double* d_F_out, double* d_cost0_out,
                                   double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                   uint8_t* d_inliers_out, void* stream);
+/* Refinement of homographies on their inliers, over a RAGGED batch laid out as above (d_offsets, d_x1y1 / d_x2y2 with
+ * only columns 0-1 used, d_mask): per pair, Levenberg-Marquardt from d_H [n_pairs][9] (row-major, x2 ~ H x1: what
+ * dgb200_find_homography_* return) on the cost C = sum of h_resid_sampson(G, row) over the rows with mask != 0, where
+ * G = H^-1 is the engine's image-2 -> image-1 model (column-major, csrc/hgeom.h).  The per-row value is the residual of
+ * the H RANSAC's default inlier rule (px^2), so a refined inlier means what a RANSAC inlier means.
+ *   Residuals for the Jacobian: with the algebraic pair e = (r1, r2) and JJ^T = [[A, B], [B, D]] of h_resid_sampson,
+ *   z1 = r1 / sqrt(A), z2 = (r2 - (B / sqrt(A)) z1) / sqrt(D - B^2 / A), so |z|^2 = e^T (JJ^T)^-1 e; analytic Jacobian.
+ *   Parameters: 8, re-centred at every accepted step, in Hartley-normalised coordinates.  T1, T2 move the masked rows
+ *   of each image to their centroid and an RMS distance of sqrt(2); the normalised model M = T1 G T2^-1 / |.|_F moves
+ *   as M <- (M + B d) / |M + B d|_F, B (9 x 8) the Householder basis of the plane orthogonal to M.  Residuals are
+ *   evaluated in pixels through G = T1^-1 M T2: the normalisation changes the conditioning, not the cost.
+ *   Schedule (that of dgb200_refine_pose_ragged_dev): lambda = 1e-3; a trial step solves (J^T J + lambda diag(J^T J))
+ *   D = -J^T z (a pivot of the 8 x 8 Cholesky factor that is not positive rejects it) and is accepted when its cost is
+ *   strictly lower (lambda <- max(lambda / 10, 1e-12)), else lambda <- 10 lambda; stops after max_iters trial steps,
+ *   after a trial step whose cost differs from the current one by less than 1e-12 of it, or when lambda > 1e8.
+ * The sums of a pair are reduced in a fixed order without atomics: its result does not depend on the batch or the run.
+ * Outputs per pair: d_H_out [9] the refined H (x2 ~ H x1), unit Frobenius norm, det H > 0 (the input H so normalised
+ * when no step was accepted); d_cost0_out, d_cost_out the cost before and after (cost <= cost0); d_n_used_out the rows
+ * with mask != 0; d_iters_out the trial steps taken.  d_inliers_out [rows], when given: h_resid_sampson(H_out^-1, row)
+ * <= px_th^2 for EVERY row of the pair, masked or not -- the comparison of the RANSAC's mask.
+ * Pairs that are not refined: fewer than 5 rows with mask != 0: H passed through (normalised as above), cost0 = cost,
+ * iters = 0.  H all zero, holding a NaN, or with an inverse that is not finite (no model): H = 0, NaN costs,
+ * n_used = iters = 0, inlier rows 0.  Offsets that decrease, are negative or pass `rows`: per-pair outputs as for no
+ * model, no row read or written.
+ * d_mask, d_cost0_out, d_n_used_out, d_iters_out and d_inliers_out may be NULL; d_x1y1 / d_x2y2 may be NULL when
+ * rows = 0; every other buffer is required.  d_H_out may be d_H (in place).  A null required buffer, n_pairs < 1,
+ * rows < 0, dim < 2, max_iters < 0, or d_inliers_out with a negative or NaN px_th returns DGB200_E_ARG before any
+ * launch.  Asynchronous on `stream`, one kernel, no workspace. */
+int dgb200_refine_homography_ragged_dev(const double* d_H, const double* d_x1y1, const double* d_x2y2,
+                                        const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                        int max_iters, double px_th, double* d_H_out, double* d_cost0_out,
+                                        double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                        uint8_t* d_inliers_out, void* stream);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

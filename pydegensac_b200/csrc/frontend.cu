@@ -12,6 +12,8 @@
 //           inliers (one warp per pair);  the reference stops at F (the survey lists E/pose as the step after).
 //           Pose and scene plane from a homography (planar scenes, pure rotations): the decompositions of
 //           K2^-1 H K1, cheirality vote, the two best candidates; the rows and median of the F path.
+//           Refinement on the inliers of the pose (Sampson error of F = K2^-T [t]x R K1^-1) and of a homography
+//           (the engine's Sampson error of H), batched Levenberg-Marquardt.
 //   ALSO    the reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594, USE_QR) as a batch
 //           kernel over many samples (la.h restates LAPACK's dgeqp3 kernel).
 #include <cuda_runtime.h>
@@ -25,6 +27,7 @@
 #include "la.h"
 #include "hgeom.h"
 #include "pose_refine.h"
+#include "refine_h.h"
 #include "rng.h"
 
 namespace {
@@ -1228,6 +1231,186 @@ __global__ void __launch_bounds__(kPoseThreads) pose_refine_ragged_kernel(PoseRe
   }
 }
 
+// ------------------------------------------------------------------------------------------------ H refinement, ragged
+struct HRefineArgs {
+  const double* H;                                         // [P][9] row-major, x2 ~ H x1
+  const double* x1y1; const double* x2y2; const int* offsets; const unsigned char* mask;   // [rows][dim], [P+1], [rows]
+  int n_pairs, rows, dim, max_iters;
+  double th2;                                              // px_th^2 of the inlier rows
+  double* H_out; double* cost0; double* cost; int* n_used; int* iters;   // [P][9], [P] (cost0, n_used, iters may be null)
+  unsigned char* inliers;                                  // [rows] or null
+};
+
+// One pass over the pair's rows with mask != 0: row(x1, y1, x2, y2, acc) adds the row's NS sums, which are reduced
+// over the CTA into out[NS], the number of rows into *count -- the fixed-shape tree of pose_refine_pass (butterfly
+// shuffles in each warp, then thread j < NS adds the warps' partials of sum j in warp order; no atomics).  Called by
+// all threads; ends with a barrier.
+template <int NS, class Row>
+__device__ __forceinline__ void h_refine_pass(const HRefineArgs& a, int r0, int n, Row row,
+                                              double (*wpart)[dg::kRhSums], int* wcount, double* out, int* count) {
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const unsigned char* mk = a.mask;
+  const double* g1 = a.x1y1;
+  const double* g2 = a.x2y2;
+  const int dim = a.dim;
+  double acc[NS];
+#pragma unroll
+  for (int j = 0; j < NS; ++j) acc[j] = 0.0;
+  int cnt = 0;
+  for (int i = tid; i < n; i += kPoseThreads) {
+    const size_t r = (size_t)r0 + i;
+    if (mk && !mk[r]) continue;
+    ++cnt;
+    row(g1[r * dim], g1[r * dim + 1], g2[r * dim], g2[r * dim + 1], acc);
+  }
+#pragma unroll
+  for (int j = 0; j < NS; ++j)
+    for (int o = 16; o > 0; o >>= 1) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if (lane == 0) {
+#pragma unroll
+    for (int j = 0; j < NS; ++j) wpart[wid][j] = acc[j];
+    wcount[wid] = cnt;
+  }
+  __syncthreads();
+  if (tid < NS) {
+    double s = wpart[0][tid];
+    for (int w = 1; w < kPoseThreads / 32; ++w) s += wpart[w][tid];
+    out[tid] = s;
+  } else if (tid == NS) {
+    int c = 0;
+    for (int w = 0; w < kPoseThreads / 32; ++w) c += wcount[w];
+    *count = c;
+  }
+  __syncthreads();
+}
+
+// Thread 0's serial part of a trial step: D of the damped normal equations (cur: the current sums), the trial model
+// M2 = M (+) D and the linearisation there into lin.  0 when the solve rejects the step.  Not inlined: the 8 x 8 factor
+// then lives in this function's frame instead of competing with the row passes for the kernel's registers.
+__device__ __noinline__ int h_refine_trial(const double* cur, double lam, const double* tr, const double* M, double* M2,
+                                           double* lin) {
+  double D[8];
+  if (!dg::pr_cholesky_solve<8>(cur + 1, cur + 37, lam, D)) return 0;
+  dg::rh_step(M, D, M2);
+  dg::rh_linearise(tr, tr + 3, M2, lin, lin + 9);
+  return 1;
+}
+
+// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1: Levenberg-Marquardt with Marquardt scaling on the
+// Sampson cost C = sum of h_resid_sampson(G, row) over the rows with mask != 0, G = H^-1 the engine's image-2 -> image-1
+// model (refine_h.h has the whitened residuals, their analytic Jacobian and the 8 local parameters).
+//   start:  thread 0 takes G = adj(H) / det(H); one pass sums x, y, x^2, y^2 of the masked rows of each image, thread 0
+//           forms T1, T2, M = T1 G T2^-1 / |.|_F and linearises there; one pass gives C, J^T J, J^T z; lambda = 1e-3.
+//   trial:  the schedule of pose_refine_ragged_kernel with an 8 x 8 Cholesky solve: (J^T J + lambda diag J^T J) D =
+//           -J^T z, a pivot that is not positive rejects the step without a pass; C' < C accepts it (lambda <-
+//           max(lambda / 10, 1e-12)), else lambda <- 10 lambda, stop when lambda > 1e8; |C - C'| < 1e-12 C stops.
+//   end:    H = adj(T1^-1 M T2) after an accepted step, else the input H; scaled to unit Frobenius norm, det H > 0.  With
+//           inliers_out one more pass over ALL the pair's rows: h_resid_sampson(H_out^-1, row) <= th2.
+// Fewer than kRhMinRows rows with mask != 0: H is passed through (normalised), cost0 = cost, iters = 0.  H all zero, a NaN
+// in H or an inverse that is not finite (no model): H = 0, NaN costs, n_used = iters = 0, inlier rows 0.  Offsets that
+// decrease, are negative or pass `rows`: the same per-pair outputs and no row is read or written.  H_out may be H: H
+// is read into shared memory before the first barrier and written after it.
+__global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineArgs a) {
+  __shared__ double hio[9];                        // the input H; at the end the output H
+  __shared__ double tr[6];                         // T1, T2 as (s, mx, my)
+  __shared__ double model[2][9];                   // current and trial M
+  __shared__ double lin[81];                       // G [9], dG [8][9] of the pass to come; at the end H_out^-1
+  __shared__ double cur[dg::kRhSums], trial[dg::kRhSums];
+  __shared__ double wpart[kPoseThreads / 32][dg::kRhSums];
+  __shared__ int wcount[kPoseThreads / 32];
+  __shared__ int s_count, s_go;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int b = a.offsets[p], e = a.offsets[p + 1];
+  const bool span_ok = b >= 0 && b <= e && e <= a.rows;
+  const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
+  if (tid < 9) hio[tid] = a.H[(size_t)p * 9 + tid];
+  __syncthreads();                                 // H is read: the outputs may overwrite it
+  if (tid == 0) s_go = dg::rh_engine_model(hio, lin) ? 1 : 0;
+  __syncthreads();
+  if (!span_ok || !s_go) {                         // (block-uniform)
+    if (a.inliers) for (int i = tid; i < n; i += kPoseThreads) a.inliers[(size_t)r0 + i] = 0;
+    if (tid < 9) a.H_out[(size_t)p * 9 + tid] = 0.0;
+    if (tid == 0) {
+      a.cost[p] = qnan();
+      if (a.cost0) a.cost0[p] = qnan();
+      if (a.n_used) a.n_used[p] = 0;
+      if (a.iters) a.iters[p] = 0;
+    }
+    return;
+  }
+  h_refine_pass<dg::kRhNormSums>(a, r0, n, [](double x1, double y1, double x2, double y2, double* acc) {
+    acc[0] += x1; acc[1] += y1; acc[2] += x1 * x1; acc[3] += y1 * y1;
+    acc[4] += x2; acc[5] += y2; acc[6] += x2 * x2; acc[7] += y2 * y2;
+  }, wpart, wcount, trial, &s_count);
+  const int n_used = s_count;
+  auto lm_row = [](const double* G, const double* dG) {
+    return [G, dG](double x1, double y1, double x2, double y2, double* acc) { dg::rh_row(G, dG, x1, y1, x2, y2, acc); };
+  };
+  if (tid == 0) {
+    dg::rh_transform(trial, n_used, tr);
+    dg::rh_transform(trial + 4, n_used, tr + 3);
+    double G[9];
+    for (int i = 0; i < 9; ++i) G[i] = lin[i];
+    dg::rh_from_pixels(tr, tr + 3, G, model[0]);
+    dg::rh_linearise(tr, tr + 3, model[0], lin, lin + 9);
+  }
+  __syncthreads();
+  h_refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, cur, &s_count);
+  const double cost0 = cur[0];
+  double lam = dg::kPrLambda0;
+  int iters = 0, accepted = 0;
+  while (n_used >= dg::kRhMinRows && iters < a.max_iters) {   // (block-uniform: every thread keeps the same lam, iters)
+    ++iters;
+    if (tid == 0) s_go = h_refine_trial(cur, lam, tr, model[0], model[1], lin);
+    __syncthreads();
+    const bool go = s_go != 0;
+    if (go) h_refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, trial, &s_count);
+    const double c_old = cur[0], c_new = trial[0];
+    const bool better = go && c_new < c_old;
+    const bool flat = go && fabs(c_old - c_new) < dg::kPrRelDecrease * c_old;   // converged: the cost no longer moves
+    __syncthreads();                               // s_go, cur[0], trial[0] are read: they may change
+    if (better) {
+      if (tid < dg::kRhSums) cur[tid] = trial[tid];
+      if (tid < 9) model[0][tid] = model[1][tid];
+    }
+    __syncthreads();
+    if (better) {
+      lam = fmax(lam / 10.0, dg::kPrLambdaMin);
+      ++accepted;
+      if (flat) break;
+    } else {
+      lam *= 10.0;
+      if (flat || lam > dg::kPrLambdaMax) break;
+    }
+  }
+  if (tid == 0) {
+    if (accepted) {
+      double G[9];
+      dg::rh_to_pixels(tr, tr + 3, model[0], G);
+      dg::rh_public_model(G, hio);
+    } else {
+      dg::rh_unit_det_pos(hio);
+    }
+    dg::rh_engine_model(hio, lin);
+  }
+  __syncthreads();
+  if (tid < 9) a.H_out[(size_t)p * 9 + tid] = hio[tid];
+  if (tid == 0) {
+    a.cost[p] = cur[0];
+    if (a.cost0) a.cost0[p] = cost0;
+    if (a.n_used) a.n_used[p] = n_used;
+    if (a.iters) a.iters[p] = iters;
+  }
+  if (a.inliers) {
+    const int dim = a.dim;
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      a.inliers[r] = dg::h_resid_sampson(lin, a.x1y1[r * dim], a.x1y1[r * dim + 1], a.x2y2[r * dim], a.x2y2[r * dim + 1]) <= a.th2;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ QR null space
 __global__ void qr7x9_kernel(const double* A, double* N, int* rc, int count) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1587,6 +1770,26 @@ int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const do
   a.R_out = d_R_out; a.t_out = d_t_out; a.F_out = d_F_out; a.cost0 = d_cost0_out; a.cost = d_cost_out;
   a.n_used = d_n_used_out; a.iters = d_iters_out; a.inliers = d_inliers_out;
   pose_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
+int dgb200_refine_homography_ragged_dev(const double* d_H, const double* d_x1y1, const double* d_x2y2,
+                                        const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                        int max_iters, double px_th, double* d_H_out, double* d_cost0_out,
+                                        double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                        uint8_t* d_inliers_out, void* stream) {
+  if (!d_H || !d_offsets || !d_H_out || !d_cost_out) return fail2(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
+  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+  HRefineArgs a;
+  a.H = d_H; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
+  a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
+  a.H_out = d_H_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
+  a.inliers = d_inliers_out;
+  h_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
   CU2(cudaGetLastError());
   return 0;
 }

@@ -108,46 +108,49 @@ DG_HD void pr_row(const double* F, const double* dF, double x1, double y1, doubl
   for (int k = 0; k < 5; ++k) acc[16 + k] += J[k] * r;
 }
 
-// D [5] of (H + lam diag(H)) D = -g by Cholesky; H: upper triangle by rows [15].  false at a pivot that is not positive.
-DG_HD bool pr_solve(const double* H, const double* g, double lam, double* D) {
-  double L[5][5];
+// D [N] of (H + lam diag(H)) D = -g by Cholesky; H: upper triangle by rows [N (N + 1) / 2].  false at a pivot that is
+// not positive.  (N = 8: the homography refinement, refine_h.h.)
+template <int N>
+DG_HD bool pr_cholesky_solve(const double* H, const double* g, double lam, double* D) {
+  double L[N][N];
   int m = 0;
 #pragma unroll
-  for (int k = 0; k < 5; ++k)
+  for (int k = 0; k < N; ++k)
 #pragma unroll
-    for (int l = k; l < 5; ++l) { L[l][k] = (l == k) ? H[m] + lam * H[m] : H[m]; ++m; }
+    for (int l = k; l < N; ++l) { L[l][k] = (l == k) ? H[m] + lam * H[m] : H[m]; ++m; }
 #pragma unroll
-  for (int j = 0; j < 5; ++j) {
+  for (int j = 0; j < N; ++j) {
     double d = L[j][j];
 #pragma unroll
     for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
     if (!(d > 0.0)) return false;
     L[j][j] = sqrt(d);
 #pragma unroll
-    for (int i = j + 1; i < 5; ++i) {
+    for (int i = j + 1; i < N; ++i) {
       double v = L[i][j];
 #pragma unroll
       for (int k = 0; k < j; ++k) v -= L[i][k] * L[j][k];
       L[i][j] = v / L[j][j];
     }
   }
-  double y[5];
+  double y[N];
 #pragma unroll
-  for (int i = 0; i < 5; ++i) {
+  for (int i = 0; i < N; ++i) {
     double v = -g[i];
 #pragma unroll
     for (int k = 0; k < i; ++k) v -= L[i][k] * y[k];
     y[i] = v / L[i][i];
   }
 #pragma unroll
-  for (int i = 4; i >= 0; --i) {
+  for (int i = N - 1; i >= 0; --i) {
     double v = y[i];
 #pragma unroll
-    for (int k = i + 1; k < 5; ++k) v -= L[k][i] * D[k];
+    for (int k = i + 1; k < N; ++k) v -= L[k][i] * D[k];
     D[i] = v / L[i][i];
   }
   return true;
 }
+DG_HD bool pr_solve(const double* H, const double* g, double lam, double* D) { return pr_cholesky_solve<5>(H, g, lam, D); }
 
 // The pose D = (w, d) away from (R, t): exp([w]x) = I + (sin a / a) [w]x + (2 sin^2(a/2) / a^2) [w]x^2, a = |w|
 DG_HD void pr_step(const double* R, const double* t, const double* D, double* R2, double* t2) {

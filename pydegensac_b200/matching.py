@@ -34,6 +34,10 @@ The H branch (planar scenes, pure rotations): pose and scene plane from H, the b
 
     H, hmask = pydegensac_b200.findHomographyBatch(m.pts1, m.pts2, 2.0, 0.999, 10000, offsets=m.offsets, n_max=m.n_max)
     hpose = pose_from_homography_ragged(H, K1, K2, m.pts1, m.pts2, m.offsets, hmask)
+
+H refined on its inliers first (Levenberg-Marquardt on the Sampson error of the H RANSAC's inlier rule):
+
+    fine_h = refine_homography_ragged(H, m.pts1, m.pts2, m.offsets, hmask, px_th=2.0)
 """
 import collections
 import ctypes
@@ -48,6 +52,7 @@ BatchLayout = collections.namedtuple("BatchLayout", "tile_prefix row_prefix col_
 BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offsets n_max")
 RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angle median_angle")
 RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used iters inliers")
+RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_used iters inliers")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -416,6 +421,81 @@ def refine_pose_ragged(R, t, K1, K2, pts1, pts2, offsets, mask=None, max_iters=1
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return RefinedPose(Ro, to, Fo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None)
+
+
+def refine_homography_ragged(H, pts1, pts2, offsets, mask=None, max_iters=10, px_th=None):
+    """Refine the homography of every pair of a ragged batch on its inliers: Levenberg-Marquardt on the Sampson error.
+
+    findHomographyBatch returns the local optimisation's iterated algebraic (DLT) fit, which minimises no geometric
+    error; this step minimises, per pair, the sum of the engine's Sampson errors over the rows with mask set -- the
+    residual of the H RANSAC's default inlier rule (error_type="sampson", px^2) -- over the 8 degrees of freedom of H,
+    starting from the H given, as cv2.findHomography polishes its result.  All inputs are CUDA tensors on one device:
+    H [P,3,3] or [P,9] (x2 ~ H x1, what findHomographyBatch returns), pts1 / pts2 [rows, 2|6] (columns 0-1 are the
+    pixel coordinates), offsets int32 [P+1], mask [rows] bool / uint8 or None (every row); floating inputs are used in
+    float64.  The intended call is refine_homography_ragged(H, m.pts1, m.pts2, m.offsets, hmask, px_th=...), straight
+    from the ragged findHomographyBatch.  max_iters bounds the trial steps per pair (schedule: include/degensac_b200.h).
+    Returns RefinedHomography(H, cost0, cost, n_used, iters, inliers): H [P,3,3] refined, unit Frobenius norm, det > 0
+    (what pose_from_homography_ragged and match_descriptors_guided(..., guide="H") take); cost0 / cost [P] the summed
+    Sampson error (px^2) before and after, cost <= cost0; n_used [P] int32 the rows used; iters [P] int32 the trial steps
+    taken; inliers [rows] bool, with px_th given: Sampson error of the refined H at most px_th^2 for every row, masked or
+    not (None without px_th).  A pair with fewer than 5 rows used keeps its H (normalised; iters 0); a pair whose H is
+    all zero, holds a NaN or is singular (no model) gets H = 0, NaN costs and no inliers.  The result of a pair does not
+    depend on the batch it is in.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("H", H), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
+    for name, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % name)
+    if H.dim() not in (2, 3) or H.shape[0] < 1 or tuple(H.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("H must be [P,3,3] or [P,9] with P >= 1, not %s" % list(H.shape))
+    P = int(H.shape[0])
+    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
+        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
+    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
+    if tuple(offsets.shape) != (P + 1,):
+        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
+    if offsets.dtype != torch.int32:
+        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
+    for name, x in (("H", H), ("pts1", pts1), ("pts2", pts2)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (rows,):
+            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    max_iters = int(max_iters)
+    if max_iters < 0:
+        raise ValueError("max_iters must not be negative, not %d" % max_iters)
+    if px_th is not None:
+        px_th = float(px_th)
+        if not px_th >= 0.0:
+            raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
+    dev = pts1.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("H, pts1, pts2, offsets and mask must be CUDA tensors on one device")
+    f64 = torch.float64
+    Hc = H.to(f64).contiguous()
+    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
+    off = offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        Ho = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        cost0 = torch.empty(P, dtype=f64, device=dev)
+        cost = torch.empty(P, dtype=f64, device=dev)
+        n_used = torch.empty(P, dtype=torch.int32, device=dev)
+        iters = torch.empty(P, dtype=torch.int32, device=dev)
+        inl = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows] if px_th is not None else None
+        vp = ctypes.c_void_p
+        rc = L.dgb200_refine_homography_ragged_dev(
+            vp(Hc.data_ptr()), vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
+            vp(m.data_ptr()) if m is not None else None, max_iters, ctypes.c_double(px_th if px_th is not None else 0.0),
+            vp(Ho.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(n_used.data_ptr()), vp(iters.data_ptr()),
+            vp(inl.data_ptr()) if inl is not None else None, vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_frontend_last_error().decode())
+    return RefinedHomography(Ho, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
