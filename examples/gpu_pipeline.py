@@ -3,6 +3,7 @@
 
     descriptors + keypoints (CUDA tensors)  ->  2-NN matching + SNN ratio test   (pydegensac_b200.matching, CUDA)
                                             ->  findHomography / findFundamentalMatrix (device-resident tensors)
+                                            ->  F refined on the inliers (Sampson error)  (pydegensac_b200.matching)
                                             ->  guided re-match inside F's epipolar band   (pydegensac_b200.matching, CUDA)
                                             ->  relative pose from F                      (pydegensac_b200.matching)
                                             ->  pose refined on the inliers (Sampson error) (pydegensac_b200.matching)
@@ -24,7 +25,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
 from pydegensac_b200.matching import (match_descriptors, match_descriptors_guided, pose_from_fundamental,
                                       pose_from_fundamental_ragged, pose_from_homography_ragged,
-                                      refine_homography_ragged, refine_pose_ragged)
+                                      refine_fundamental_ragged, refine_homography_ragged, refine_pose_ragged)
 from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
@@ -60,14 +61,20 @@ def main():
     print("tentative correspondences:", len(idx1))
     F, mask = pydegensac.findFundamentalMatrixBatch(pts1[None], pts2[None], 0.5, 0.999, 50000, seeds=[0])
     print("pydegensac_b200 found %d inliers" % int(mask.sum()))
-    # guided re-match: candidates of a query are the train keypoints within 1 px (Sampson) of its epipolar line
-    g = match_descriptors_guided([d1, d2], [[0, 1]], [kp1, kp2], F, 1.0, guide="F", ratio=0.9)
+    # F refined on its inliers (Sampson error over the rank-2 matrices, no intrinsics needed), through the ragged entry
+    # points with one pair
+    offsets = torch.tensor([0, len(idx1)], dtype=torch.int32, device=dev)
+    ff = refine_fundamental_ragged(F, pts1, pts2, offsets, mask[0], px_th=1.0)
+    print("F refined on %d rows in %d trial steps: summed Sampson error %.3f -> %.3f px^2, %d inliers at 1 px"
+          % (int(ff.n_used[0]), int(ff.iters[0]), float(ff.cost0[0]), float(ff.cost[0]), int(ff.inliers.sum())))
+    # guided re-match: candidates of a query are the train keypoints within 1 px (Sampson) of its epipolar line under
+    # the refined F
+    g = match_descriptors_guided([d1, d2], [[0, 1]], [kp1, kp2], ff.F, 1.0, guide="F", ratio=0.9)
     print("tentative correspondences: %d unguided, %d guided by F" % (len(idx1), int(g.offsets[1])))
     K = torch.from_numpy(_K).to(dev)
     R, t, good = pose_from_fundamental(F, K, K, pts1[None], pts2[None], mask)
     print("R =\n", R[0].cpu().numpy(), "\nt =", t[0].cpu().numpy(), " (%d correspondences in front of both cameras)" % int(good[0]))
-    # refinement on the inliers in front of both cameras, through the ragged entry points with one pair
-    offsets = torch.tensor([0, len(idx1)], dtype=torch.int32, device=dev)
+    # refinement of the pose on the inliers in front of both cameras
     pose = pose_from_fundamental_ragged(F, K, K, pts1, pts2, offsets, mask[0])
     fine = refine_pose_ragged(pose.R, pose.t, K, K, pts1, pts2, offsets, pose.in_front, px_th=0.5)
     print("refined on %d rows in %d trial steps: sum of squared Sampson residuals %.3f -> %.3f px^2, %d inliers at 0.5 px"

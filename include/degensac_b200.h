@@ -369,6 +369,42 @@ int dgb200_refine_homography_ragged_dev(const double* d_H, const double* d_x1y1,
                                         int max_iters, double px_th, double* d_H_out, double* d_cost0_out,
                                         double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                         uint8_t* d_inliers_out, void* stream);
+/* Refinement of fundamental matrices on their inliers, for pairs whose intrinsics are unknown, over a RAGGED batch laid
+ * out as above (d_offsets, d_x1y1 / d_x2y2 with only columns 0-1 used, d_mask): per pair, Levenberg-Marquardt from
+ * d_F [n_pairs][9] (row-major, x2^T F x1 = 0: what dgb200_find_fundamental_* return) on the cost C = sum of
+ * f_resid_sampson(F, row) over the rows with mask != 0 -- the residual of the F RANSAC's default inlier rule (px^2), so
+ * a refined inlier means what a RANSAC inlier means.  Gauss-Newton residual r = (p2^T F p1) / sqrt(s), r^2 the Sampson
+ * error, independent of the scale of F; analytic Jacobian.
+ *   Parameters: 7, re-centred at every accepted step, in Hartley-normalised coordinates, over the rank-2 matrices.
+ *   T1, T2 move the masked rows of each image to their centroid and an RMS distance of sqrt(2); the normalised model is
+ *   Fn = T2^-T F T1^-1 at unit Frobenius norm, starting from Fn0 = unit(rank2(T2^-T F_in T1^-1)) (F_in itself, up to
+ *   rounding, when it has rank 2; a full-rank F_in is projected).  A step is Fn <- unit(rank2(Fn + B d)), rank2 the
+ *   projection that zeroes the smallest singular value, and B (9 x 7) an orthonormal basis of the complement of vec(Fn)
+ *   and vec(cof Fn) -- the tangent space of the unit-norm rank-2 matrices at Fn -- built by two Householder
+ *   reflections, so it has no gauge direction and depends on Fn alone.  Residuals are evaluated in pixels through
+ *   F = T2^T Fn T1: the normalisation changes the conditioning, not the cost.
+ *   Schedule (that of dgb200_refine_pose_ragged_dev): lambda = 1e-3; a trial step solves (J^T J + lambda diag(J^T J))
+ *   D = -J^T r (a pivot of the 7 x 7 Cholesky factor that is not positive rejects it) and is accepted when its cost is
+ *   strictly lower (lambda <- max(lambda / 10, 1e-12)), else lambda <- 10 lambda; stops after max_iters trial steps,
+ *   after a trial step whose cost differs from the current one by less than 1e-12 of it, or when lambda > 1e8.
+ * The sums of a pair are reduced in a fixed order without atomics: its result does not depend on the batch or the run.
+ * Outputs per pair: d_F_out [9] the refined F = T2^T Fn T1 (x2^T F x1 = 0, row-major), rank 2, unit Frobenius norm,
+ * signed so that <F_out, F_in> >= 0 (the start point so mapped back when no step was accepted); d_cost0_out, d_cost_out
+ * the cost at the start point and after (cost <= cost0); d_n_used_out the rows with mask != 0; d_iters_out the trial
+ * steps taken.  d_inliers_out [rows], when given: f_resid_sampson(F_out, row) <= px_th^2 for EVERY row of the pair,
+ * masked or not -- the comparison of the RANSAC's mask.
+ * Pairs that are not refined: fewer than 8 rows with mask != 0: the start point passed through (as above), cost0 = cost,
+ * iters = 0.  F all zero or holding a value that is not finite (no model): F = 0, NaN costs, n_used = iters = 0, inlier
+ * rows 0.  Offsets that decrease, are negative or pass `rows`: per-pair outputs as for no model, no row read or written.
+ * d_mask, d_cost0_out, d_n_used_out, d_iters_out and d_inliers_out may be NULL; d_x1y1 / d_x2y2 may be NULL when
+ * rows = 0; every other buffer is required.  d_F_out may be d_F (in place).  A null required buffer, n_pairs < 1,
+ * rows < 0, dim < 2, max_iters < 0, or d_inliers_out with a negative or NaN px_th returns DGB200_E_ARG before any
+ * launch.  Asynchronous on `stream`, one kernel, no workspace. */
+int dgb200_refine_fundamental_ragged_dev(const double* d_F, const double* d_x1y1, const double* d_x2y2,
+                                         const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                         int max_iters, double px_th, double* d_F_out, double* d_cost0_out,
+                                         double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                         uint8_t* d_inliers_out, void* stream);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

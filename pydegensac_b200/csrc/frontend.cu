@@ -12,8 +12,9 @@
 //           inliers (one warp per pair);  the reference stops at F (the survey lists E/pose as the step after).
 //           Pose and scene plane from a homography (planar scenes, pure rotations): the decompositions of
 //           K2^-1 H K1, cheirality vote, the two best candidates; the rows and median of the F path.
-//           Refinement on the inliers of the pose (Sampson error of F = K2^-T [t]x R K1^-1) and of a homography
-//           (the engine's Sampson error of H), batched Levenberg-Marquardt.
+//           Refinement on the inliers of the pose (Sampson error of F = K2^-T [t]x R K1^-1), of a homography
+//           (the engine's Sampson error of H) and of a fundamental matrix (its Sampson error over the rank-2
+//           matrices), batched Levenberg-Marquardt.
 //   ALSO    the reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594, USE_QR) as a batch
 //           kernel over many samples (la.h restates LAPACK's dgeqp3 kernel).
 #include <cuda_runtime.h>
@@ -28,6 +29,7 @@
 #include "hgeom.h"
 #include "pose_refine.h"
 #include "refine_h.h"
+#include "refine_f.h"
 #include "rng.h"
 
 namespace {
@@ -1232,22 +1234,23 @@ __global__ void __launch_bounds__(kPoseThreads) pose_refine_ragged_kernel(PoseRe
 }
 
 // ------------------------------------------------------------------------------------------------ H refinement, ragged
-struct HRefineArgs {
-  const double* H;                                         // [P][9] row-major, x2 ~ H x1
+// The arguments of the H and F refinements: a 3 x 3 model per pair and its ragged rows
+struct RefineArgs {
+  const double* model;                                     // [P][9] row-major: H (x2 ~ H x1) or F (x2^T F x1 = 0)
   const double* x1y1; const double* x2y2; const int* offsets; const unsigned char* mask;   // [rows][dim], [P+1], [rows]
   int n_pairs, rows, dim, max_iters;
   double th2;                                              // px_th^2 of the inlier rows
-  double* H_out; double* cost0; double* cost; int* n_used; int* iters;   // [P][9], [P] (cost0, n_used, iters may be null)
+  double* model_out; double* cost0; double* cost; int* n_used; int* iters;   // [P][9], [P] (cost0, n_used, iters may be null)
   unsigned char* inliers;                                  // [rows] or null
 };
 
 // One pass over the pair's rows with mask != 0: row(x1, y1, x2, y2, acc) adds the row's NS sums, which are reduced
 // over the CTA into out[NS], the number of rows into *count -- the fixed-shape tree of pose_refine_pass (butterfly
 // shuffles in each warp, then thread j < NS adds the warps' partials of sum j in warp order; no atomics).  Called by
-// all threads; ends with a barrier.
+// all threads; ends with a barrier.  wpart holds the largest NS of its callers, the 45 sums of the H refinement.
 template <int NS, class Row>
-__device__ __forceinline__ void h_refine_pass(const HRefineArgs& a, int r0, int n, Row row,
-                                              double (*wpart)[dg::kRhSums], int* wcount, double* out, int* count) {
+__device__ __forceinline__ void refine_pass(const RefineArgs& a, int r0, int n, Row row,
+                                            double (*wpart)[dg::kRhSums], int* wcount, double* out, int* count) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
   const unsigned char* mk = a.mask;
   const double* g1 = a.x1y1;
@@ -1285,6 +1288,14 @@ __device__ __forceinline__ void h_refine_pass(const HRefineArgs& a, int r0, int 
   __syncthreads();
 }
 
+// The row of the first pass of both refinements: the sums x, y, x^2, y^2 of each image that rh_transform takes
+struct RefineNormRow {
+  __device__ __forceinline__ void operator()(double x1, double y1, double x2, double y2, double* acc) const {
+    acc[0] += x1; acc[1] += y1; acc[2] += x1 * x1; acc[3] += y1 * y1;
+    acc[4] += x2; acc[5] += y2; acc[6] += x2 * x2; acc[7] += y2 * y2;
+  }
+};
+
 // Thread 0's serial part of a trial step: D of the damped normal equations (cur: the current sums), the trial model
 // M2 = M (+) D and the linearisation there into lin.  0 when the solve rejects the step.  Not inlined: the 8 x 8 factor
 // then lives in this function's frame instead of competing with the row passes for the kernel's registers.
@@ -1311,7 +1322,7 @@ __device__ __noinline__ int h_refine_trial(const double* cur, double lam, const 
 // in H or an inverse that is not finite (no model): H = 0, NaN costs, n_used = iters = 0, inlier rows 0.  Offsets that
 // decrease, are negative or pass `rows`: the same per-pair outputs and no row is read or written.  H_out may be H: H
 // is read into shared memory before the first barrier and written after it.
-__global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineArgs a) {
+__global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(RefineArgs a) {
   __shared__ double hio[9];                        // the input H; at the end the output H
   __shared__ double tr[6];                         // T1, T2 as (s, mx, my)
   __shared__ double model[2][9];                   // current and trial M
@@ -1324,13 +1335,13 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
   const int b = a.offsets[p], e = a.offsets[p + 1];
   const bool span_ok = b >= 0 && b <= e && e <= a.rows;
   const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
-  if (tid < 9) hio[tid] = a.H[(size_t)p * 9 + tid];
+  if (tid < 9) hio[tid] = a.model[(size_t)p * 9 + tid];
   __syncthreads();                                 // H is read: the outputs may overwrite it
   if (tid == 0) s_go = dg::rh_engine_model(hio, lin) ? 1 : 0;
   __syncthreads();
   if (!span_ok || !s_go) {                         // (block-uniform)
     if (a.inliers) for (int i = tid; i < n; i += kPoseThreads) a.inliers[(size_t)r0 + i] = 0;
-    if (tid < 9) a.H_out[(size_t)p * 9 + tid] = 0.0;
+    if (tid < 9) a.model_out[(size_t)p * 9 + tid] = 0.0;
     if (tid == 0) {
       a.cost[p] = qnan();
       if (a.cost0) a.cost0[p] = qnan();
@@ -1339,10 +1350,7 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
     }
     return;
   }
-  h_refine_pass<dg::kRhNormSums>(a, r0, n, [](double x1, double y1, double x2, double y2, double* acc) {
-    acc[0] += x1; acc[1] += y1; acc[2] += x1 * x1; acc[3] += y1 * y1;
-    acc[4] += x2; acc[5] += y2; acc[6] += x2 * x2; acc[7] += y2 * y2;
-  }, wpart, wcount, trial, &s_count);
+  refine_pass<dg::kRhNormSums>(a, r0, n, RefineNormRow(), wpart, wcount, trial, &s_count);
   const int n_used = s_count;
   auto lm_row = [](const double* G, const double* dG) {
     return [G, dG](double x1, double y1, double x2, double y2, double* acc) { dg::rh_row(G, dG, x1, y1, x2, y2, acc); };
@@ -1356,7 +1364,7 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
     dg::rh_linearise(tr, tr + 3, model[0], lin, lin + 9);
   }
   __syncthreads();
-  h_refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, cur, &s_count);
+  refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, cur, &s_count);
   const double cost0 = cur[0];
   double lam = dg::kPrLambda0;
   int iters = 0, accepted = 0;
@@ -1365,7 +1373,7 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
     if (tid == 0) s_go = h_refine_trial(cur, lam, tr, model[0], model[1], lin);
     __syncthreads();
     const bool go = s_go != 0;
-    if (go) h_refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, trial, &s_count);
+    if (go) refine_pass<dg::kRhSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, trial, &s_count);
     const double c_old = cur[0], c_new = trial[0];
     const bool better = go && c_new < c_old;
     const bool flat = go && fabs(c_old - c_new) < dg::kPrRelDecrease * c_old;   // converged: the cost no longer moves
@@ -1395,7 +1403,7 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
     dg::rh_engine_model(hio, lin);
   }
   __syncthreads();
-  if (tid < 9) a.H_out[(size_t)p * 9 + tid] = hio[tid];
+  if (tid < 9) a.model_out[(size_t)p * 9 + tid] = hio[tid];
   if (tid == 0) {
     a.cost[p] = cur[0];
     if (a.cost0) a.cost0[p] = cost0;
@@ -1407,6 +1415,119 @@ __global__ void __launch_bounds__(kPoseThreads) h_refine_ragged_kernel(HRefineAr
     for (int i = tid; i < n; i += kPoseThreads) {
       const size_t r = (size_t)r0 + i;
       a.inliers[r] = dg::h_resid_sampson(lin, a.x1y1[r * dim], a.x1y1[r * dim + 1], a.x2y2[r * dim], a.x2y2[r * dim + 1]) <= a.th2;
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ F refinement, ragged
+// Thread 0's serial part of a trial step: D of the damped normal equations (cur: the current sums), the trial model
+// Fn2 = unit(rank2(Fn + B D)) and the linearisation there into lin.  0 when the solve rejects the step.  Not inlined,
+// as h_refine_trial: the 7 x 7 factor and the rank-2 projection live in this function's frame.
+__device__ __noinline__ int f_refine_trial(const double* cur, double lam, const double* tr, const double* Fn, double* Fn2,
+                                           double* lin) {
+  double D[7];
+  if (!dg::pr_cholesky_solve<7>(cur + 1, cur + 29, lam, D)) return 0;
+  dg::rf_retract(Fn, D, Fn2);
+  dg::rf_linearise(tr, tr + 3, Fn2, lin, lin + 9);
+  return 1;
+}
+
+// Thread 0's start: T1, T2 from the sums ns [8] of n rows, the start point Fn0 = unit(rank2(T2^-T F T1^-1)) and the
+// linearisation there into lin.  Not inlined, as f_refine_trial.
+__device__ __noinline__ void f_refine_start(const double* ns, int n, const double* F, double* tr, double* Fn,
+                                            double* lin) {
+  dg::rh_transform(ns, n, tr);
+  dg::rh_transform(ns + 4, n, tr + 3);
+  dg::rf_start(tr, tr + 3, F, Fn);
+  dg::rf_linearise(tr, tr + 3, Fn, lin, lin + 9);
+}
+
+// One CTA per pair p, rows b = offsets[p] .. e = offsets[p+1]-1: Levenberg-Marquardt with Marquardt scaling on the
+// Sampson cost C = sum of f_resid_sampson(F, row) over the rows with mask != 0 (refine_f.h has the normalisation, the
+// 7 local parameters over the rank-2 matrices and the retraction; the residual and its Jacobian are pr_row's).
+//   start:  one pass sums x, y, x^2, y^2 of the masked rows of each image; thread 0 forms T1, T2, the start point
+//           Fn0 = unit(rank2(T2^-T F T1^-1)) and linearises there; one pass gives C, J^T J, J^T r; lambda = 1e-3.
+//   trial:  the schedule of h_refine_ragged_kernel with a 7 x 7 Cholesky solve and the step Fn <- unit(rank2(Fn + B d)).
+//   end:    F = T2^T Fn T1 at unit Frobenius norm, signed so that <F, F_in> >= 0 (the start point when no step was
+//           accepted).  With inliers_out one more pass over ALL the pair's rows: f_resid_sampson(F_out, row) <= th2.
+// Fewer than kRfMinRows rows with mask != 0: the start point is passed through, cost0 = cost, iters = 0.  F all zero or
+// not finite (no model): F = 0, NaN costs, n_used = iters = 0, inlier rows 0.  Offsets that decrease, are negative or
+// pass `rows`: the same per-pair outputs and no row is read or written.  F_out may be F: F is read into shared memory
+// before the first barrier and written after it.
+__global__ void __launch_bounds__(kPoseThreads) f_refine_ragged_kernel(RefineArgs a) {
+  __shared__ double fin[9];                        // the input F
+  __shared__ double tr[6];                         // T1, T2 as (s, mx, my)
+  __shared__ double model[2][9];                   // current and trial Fn
+  __shared__ double lin[72];                       // F [9], dF [7][9] of the pass to come; at the end the output F
+  __shared__ double cur[dg::kRfSums], trial[dg::kRfSums];
+  __shared__ double wpart[kPoseThreads / 32][dg::kRhSums];
+  __shared__ int wcount[kPoseThreads / 32];
+  __shared__ int s_count, s_go;
+  const int p = blockIdx.x, tid = threadIdx.x;
+  const int b = a.offsets[p], e = a.offsets[p + 1];
+  const bool span_ok = b >= 0 && b <= e && e <= a.rows;
+  const int r0 = span_ok ? b : 0, n = span_ok ? e - b : 0;
+  if (tid < 9) fin[tid] = a.model[(size_t)p * 9 + tid];
+  __syncthreads();                                 // F is read: the outputs may overwrite it
+  if (!span_ok || !dg::rf_has_model(fin)) {        // (block-uniform)
+    if (a.inliers) for (int i = tid; i < n; i += kPoseThreads) a.inliers[(size_t)r0 + i] = 0;
+    if (tid < 9) a.model_out[(size_t)p * 9 + tid] = 0.0;
+    if (tid == 0) {
+      a.cost[p] = qnan();
+      if (a.cost0) a.cost0[p] = qnan();
+      if (a.n_used) a.n_used[p] = 0;
+      if (a.iters) a.iters[p] = 0;
+    }
+    return;
+  }
+  refine_pass<dg::kRhNormSums>(a, r0, n, RefineNormRow(), wpart, wcount, trial, &s_count);
+  const int n_used = s_count;
+  auto lm_row = [](const double* F, const double* dF) {
+    return [F, dF](double x1, double y1, double x2, double y2, double* acc) { dg::pr_row_n<7, true>(F, dF, x1, y1, x2, y2, acc); };
+  };
+  if (tid == 0) f_refine_start(trial, n_used, fin, tr, model[0], lin);
+  __syncthreads();
+  refine_pass<dg::kRfSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, cur, &s_count);
+  const double cost0 = cur[0];
+  double lam = dg::kPrLambda0;
+  int iters = 0;
+  while (n_used >= dg::kRfMinRows && iters < a.max_iters) {   // (block-uniform: every thread keeps the same lam, iters)
+    ++iters;
+    if (tid == 0) s_go = f_refine_trial(cur, lam, tr, model[0], model[1], lin);
+    __syncthreads();
+    const bool go = s_go != 0;
+    if (go) refine_pass<dg::kRfSums>(a, r0, n, lm_row(lin, lin + 9), wpart, wcount, trial, &s_count);
+    const double c_old = cur[0], c_new = trial[0];
+    const bool better = go && c_new < c_old;
+    const bool flat = go && fabs(c_old - c_new) < dg::kPrRelDecrease * c_old;   // converged: the cost no longer moves
+    __syncthreads();                               // s_go, cur[0], trial[0] are read: they may change
+    if (better) {
+      if (tid < dg::kRfSums) cur[tid] = trial[tid];
+      if (tid < 9) model[0][tid] = model[1][tid];
+    }
+    __syncthreads();
+    if (better) {
+      lam = fmax(lam / 10.0, dg::kPrLambdaMin);
+      if (flat) break;
+    } else {
+      lam *= 10.0;
+      if (flat || lam > dg::kPrLambdaMax) break;
+    }
+  }
+  if (tid == 0) dg::rf_output(tr, tr + 3, model[0], fin, lin);
+  __syncthreads();
+  if (tid < 9) a.model_out[(size_t)p * 9 + tid] = lin[tid];
+  if (tid == 0) {
+    a.cost[p] = cur[0];
+    if (a.cost0) a.cost0[p] = cost0;
+    if (a.n_used) a.n_used[p] = n_used;
+    if (a.iters) a.iters[p] = iters;
+  }
+  if (a.inliers) {
+    const int dim = a.dim;
+    for (int i = tid; i < n; i += kPoseThreads) {
+      const size_t r = (size_t)r0 + i;
+      a.inliers[r] = dg::f_resid_sampson(lin, a.x1y1[r * dim], a.x1y1[r * dim + 1], a.x2y2[r * dim], a.x2y2[r * dim + 1]) <= a.th2;
     }
   }
 }
@@ -1784,12 +1905,32 @@ int dgb200_refine_homography_ragged_dev(const double* d_H, const double* d_x1y1,
   if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
   if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
   if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
-  HRefineArgs a;
-  a.H = d_H; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
+  RefineArgs a;
+  a.model = d_H; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
   a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
-  a.H_out = d_H_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
+  a.model_out = d_H_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
   a.inliers = d_inliers_out;
   h_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
+  CU2(cudaGetLastError());
+  return 0;
+}
+
+int dgb200_refine_fundamental_ragged_dev(const double* d_F, const double* d_x1y1, const double* d_x2y2,
+                                         const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask,
+                                         int max_iters, double px_th, double* d_F_out, double* d_cost0_out,
+                                         double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
+                                         uint8_t* d_inliers_out, void* stream) {
+  if (!d_F || !d_offsets || !d_F_out || !d_cost_out) return fail2(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
+  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+  RefineArgs a;
+  a.model = d_F; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
+  a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
+  a.model_out = d_F_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
+  a.inliers = d_inliers_out;
+  f_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
   CU2(cudaGetLastError());
   return 0;
 }

@@ -80,19 +80,38 @@ DG_HD void pr_linearise(const double* R, const double* t, const double* A, const
   }
 }
 
-// One correspondence at the linearisation (F, dF): adds its r^2 to acc[0] (the operations of f_resid_sampson), J_k J_l
-// (k <= l) to acc[1 .. 15] and J_k r to acc[16 .. 20], with J_k = dr/dtheta_k = dc_k / sqrt(s) - c (ds_k / 2) / (s sqrt(s)),
-// dc_k = p2^T dF_k p1, ds_k / 2 = (F p1)_{0,1} . (dF_k p1)_{0,1} + (F^T p2)_{0,1} . (dF_k^T p2)_{0,1}.
-DG_HD void pr_row(const double* F, const double* dF, double x1, double y1, double x2, double y2, double* acc) {
-  const FRes q = f_res_terms(F, x1, y1, x2, y2);
+// 9 entries of a linearisation in shared memory at p: p itself, or with kReread (device code) a copy in buf by a read
+// that the compiler may not hoist out of the row loop -- 7 x 9 derivatives kept in registers across rows take the
+// registers the sums need, and spill.
+template <bool kReread>
+DG_HD const double* pr_lin9(const double* p, double* buf) {
+  if constexpr (kReread && DG_DEVICE_PASS) {
+#pragma unroll
+    for (int i = 0; i < 9; ++i) buf[i] = *(const volatile double*)(p + i);
+    return buf;
+  } else {
+    return p;
+  }
+}
+
+// One correspondence at the linearisation (F, dF [N][9]): adds its r^2 to acc[0] (the operations of f_resid_sampson),
+// J_k J_l (k <= l) to acc[1 .. N (N + 1) / 2] and J_k r to the N sums after them, with J_k = dr/dtheta_k = dc_k / sqrt(s)
+// - c (ds_k / 2) / (s sqrt(s)), dc_k = p2^T dF_k p1, ds_k / 2 = (F p1)_{0,1} . (dF_k p1)_{0,1} + (F^T p2)_{0,1} .
+// (dF_k^T p2)_{0,1}.  (N = 7: the fundamental-matrix refinement, refine_f.h.)  With kReread the linearisation is read
+// afresh for each row (pr_lin9), as the F refinement needs it.
+template <int N, bool kReread = false>
+DG_HD void pr_row_n(const double* F, const double* dF, double x1, double y1, double x2, double y2, double* acc) {
+  double fbuf[9];
+  const FRes q = f_res_terms(pr_lin9<kReread>(F, fbuf), x1, y1, x2, y2);
   const double s = q.rxc * q.rxc + q.ryc * q.ryc + q.rx * q.rx + q.ry * q.ry;
   acc[0] += q.r * q.r / s;
   const double inv = 1.0 / sqrt(s);
   const double r = q.r * inv, w = r * inv * inv;
-  double J[5];
+  double J[N];
 #pragma unroll
-  for (int k = 0; k < 5; ++k) {
-    const double* d = dF + 9 * k;
+  for (int k = 0; k < N; ++k) {
+    double dbuf[9];
+    const double* d = pr_lin9<kReread>(dF + 9 * k, dbuf);
     const double u0 = d[0] * x1 + d[1] * y1 + d[2], u1 = d[3] * x1 + d[4] * y1 + d[5], u2 = d[6] * x1 + d[7] * y1 + d[8];
     const double v0 = d[0] * x2 + d[3] * y2 + d[6], v1 = d[1] * x2 + d[4] * y2 + d[7];
     const double dc = x2 * u0 + y2 * u1 + u2;
@@ -101,11 +120,14 @@ DG_HD void pr_row(const double* F, const double* dF, double x1, double y1, doubl
   }
   int m = 1;
 #pragma unroll
-  for (int k = 0; k < 5; ++k)
+  for (int k = 0; k < N; ++k)
 #pragma unroll
-    for (int l = k; l < 5; ++l) acc[m++] += J[k] * J[l];
+    for (int l = k; l < N; ++l) acc[m++] += J[k] * J[l];
 #pragma unroll
-  for (int k = 0; k < 5; ++k) acc[16 + k] += J[k] * r;
+  for (int k = 0; k < N; ++k) acc[1 + N * (N + 1) / 2 + k] += J[k] * r;
+}
+DG_HD void pr_row(const double* F, const double* dF, double x1, double y1, double x2, double y2, double* acc) {
+  pr_row_n<5>(F, dF, x1, y1, x2, y2, acc);
 }
 
 // D [N] of (H + lam diag(H)) D = -g by Cholesky; H: upper triangle by rows [N (N + 1) / 2].  false at a pivot that is

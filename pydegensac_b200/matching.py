@@ -38,6 +38,12 @@ The H branch (planar scenes, pure rotations): pose and scene plane from H, the b
 H refined on its inliers first (Levenberg-Marquardt on the Sampson error of the H RANSAC's inlier rule):
 
     fine_h = refine_homography_ragged(H, m.pts1, m.pts2, m.offsets, hmask, px_th=2.0)
+
+F refined on its inliers when the intrinsics are unknown (Levenberg-Marquardt on the Sampson error over the rank-2
+matrices), then the guided re-match in the band of the refined F:
+
+    fine_f = refine_fundamental_ragged(F, m.pts1, m.pts2, m.offsets, mask, px_th=1.0)
+    g = match_descriptors_guided(descs, pairs, kps, fine_f.F, 1.0, guide="F")
 """
 import collections
 import ctypes
@@ -53,6 +59,7 @@ BatchMatches = collections.namedtuple("BatchMatches", "idx1 idx2 pts1 pts2 offse
 RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angle median_angle")
 RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used iters inliers")
 RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_used iters inliers")
+RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost n_used iters inliers")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -441,14 +448,48 @@ def refine_homography_ragged(H, pts1, pts2, offsets, mask=None, max_iters=10, px
     not (None without px_th).  A pair with fewer than 5 rows used keeps its H (normalised; iters 0); a pair whose H is
     all zero, holds a NaN or is singular (no model) gets H = 0, NaN costs and no inliers.  The result of a pair does not
     depend on the batch it is in.  Asynchronous, nothing is read back."""
+    Ho, cost0, cost, n_used, iters, inl = _refine_model_ragged("H", "dgb200_refine_homography_ragged_dev", H, pts1, pts2,
+                                                               offsets, mask, max_iters, px_th)
+    return RefinedHomography(Ho, cost0, cost, n_used, iters, inl)
+
+
+def refine_fundamental_ragged(F, pts1, pts2, offsets, mask=None, max_iters=10, px_th=None):
+    """Refine the fundamental matrix of every pair of a ragged batch on its inliers: Levenberg-Marquardt on the Sampson
+    error over the rank-2 matrices, for pairs whose intrinsics are unknown.
+
+    findFundamentalMatrixBatch returns the local optimisation's iterated, weighted algebraic fit with a rank-2
+    projection, which minimises no geometric error; this step minimises, per pair, the sum of the Sampson errors over
+    the rows with mask set -- the residual of the F RANSAC's default inlier rule (error_type="sampson", px^2) -- over the
+    7 degrees of freedom of F, starting from the F given, as cv2.findFundamentalMat polishes its result.  All inputs are
+    CUDA tensors on one device: F [P,3,3] or [P,9] (x2^T F x1 = 0, what findFundamentalMatrixBatch returns), pts1 / pts2
+    [rows, 2|6] (columns 0-1 are the pixel coordinates), offsets int32 [P+1], mask [rows] bool / uint8 or None (every
+    row); floating inputs are used in float64.  The intended call is refine_fundamental_ragged(F, m.pts1, m.pts2,
+    m.offsets, mask, px_th=...), straight from the ragged findFundamentalMatrixBatch.  max_iters bounds the trial steps
+    per pair (schedule: include/degensac_b200.h).  Returns RefinedFundamental(F, cost0, cost, n_used, iters, inliers):
+    F [P,3,3] refined, rank 2, unit Frobenius norm, signed so that its inner product with the F given is not negative
+    (what match_descriptors_guided(..., guide="F") and pose_from_fundamental_ragged take); cost0 / cost [P] the summed
+    Sampson error (px^2) at the start point (the F given, projected to rank 2 if it is not) and after, cost <= cost0;
+    n_used [P] int32 the rows used; iters [P] int32 the trial steps taken; inliers [rows] bool, with px_th given:
+    Sampson error of the refined F at most px_th^2 for every row, masked or not (None without px_th).  A pair with fewer
+    than 8 rows used keeps its F (normalised; iters 0); a pair whose F is all zero or not finite (no model) gets F = 0,
+    NaN costs and no inliers.  The result of a pair does not depend on the batch it is in.  Asynchronous, nothing is
+    read back."""
+    Fo, cost0, cost, n_used, iters, inl = _refine_model_ragged("F", "dgb200_refine_fundamental_ragged_dev", F, pts1,
+                                                               pts2, offsets, mask, max_iters, px_th)
+    return RefinedFundamental(Fo, cost0, cost, n_used, iters, inl)
+
+
+def _refine_model_ragged(name, entry, M, pts1, pts2, offsets, mask, max_iters, px_th):
+    """The checks and the call of a refinement of one 3 x 3 model per pair (H or F, by `name`) through the C entry
+    point `entry`: the refined models [P,3,3], cost0, cost, n_used, iters and the inlier rows (None without px_th)."""
     import torch
-    named = (("H", H), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
-    for name, x in named + ((("mask", mask),) if mask is not None else ()):
+    named = ((name, M), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
         if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % name)
-    if H.dim() not in (2, 3) or H.shape[0] < 1 or tuple(H.shape[1:]) not in ((3, 3), (9,)):
-        raise ValueError("H must be [P,3,3] or [P,9] with P >= 1, not %s" % list(H.shape))
-    P = int(H.shape[0])
+            raise ValueError("%s must be a torch tensor" % nm)
+    if M.dim() not in (2, 3) or M.shape[0] < 1 or tuple(M.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("%s must be [P,3,3] or [P,9] with P >= 1, not %s" % (name, list(M.shape)))
+    P = int(M.shape[0])
     if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
         raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
     rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
@@ -456,9 +497,9 @@ def refine_homography_ragged(H, pts1, pts2, offsets, mask=None, max_iters=10, px
         raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
     if offsets.dtype != torch.int32:
         raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    for name, x in (("H", H), ("pts1", pts1), ("pts2", pts2)):
+    for nm, x in ((name, M), ("pts1", pts1), ("pts2", pts2)):
         if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
     if mask is not None:
         if tuple(mask.shape) != (rows,):
             raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
@@ -473,29 +514,29 @@ def refine_homography_ragged(H, pts1, pts2, offsets, mask=None, max_iters=10, px
             raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
     dev = pts1.device
     if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("H, pts1, pts2, offsets and mask must be CUDA tensors on one device")
+        raise ValueError("%s, pts1, pts2, offsets and mask must be CUDA tensors on one device" % name)
     f64 = torch.float64
-    Hc = H.to(f64).contiguous()
+    Mc = M.to(f64).contiguous()
     p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
     off = offsets.contiguous()
     m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
     with torch.cuda.device(dev):
-        Ho = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        Mo = torch.empty((P, 3, 3), dtype=f64, device=dev)
         cost0 = torch.empty(P, dtype=f64, device=dev)
         cost = torch.empty(P, dtype=f64, device=dev)
         n_used = torch.empty(P, dtype=torch.int32, device=dev)
         iters = torch.empty(P, dtype=torch.int32, device=dev)
         inl = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows] if px_th is not None else None
         vp = ctypes.c_void_p
-        rc = L.dgb200_refine_homography_ragged_dev(
-            vp(Hc.data_ptr()), vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
+        rc = getattr(L, entry)(
+            vp(Mc.data_ptr()), vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
             vp(m.data_ptr()) if m is not None else None, max_iters, ctypes.c_double(px_th if px_th is not None else 0.0),
-            vp(Ho.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(n_used.data_ptr()), vp(iters.data_ptr()),
+            vp(Mo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(n_used.data_ptr()), vp(iters.data_ptr()),
             vp(inl.data_ptr()) if inl is not None else None, vp(torch.cuda.current_stream(dev).cuda_stream))
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
-    return RefinedHomography(Ho, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None)
+    return Mo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
