@@ -8,6 +8,8 @@
                                             ->  relative pose from F                      (pydegensac_b200.matching)
                                             ->  pose refined on the inliers (Sampson error) (pydegensac_b200.matching)
     and the H branch for a planar scene:    ->  findHomographyBatch -> pose and scene plane from H
+    and a third view:                       ->  its matches to view 0 carry the two-view points (scatter / gather)
+                                            ->  absolute pose by P3P RANSAC                (pydegensac_b200.matching)
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -23,9 +25,10 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (match_descriptors, match_descriptors_guided, pose_from_fundamental,
-                                      pose_from_fundamental_ragged, pose_from_homography_ragged,
-                                      refine_fundamental_ragged, refine_homography_ragged, refine_pose_ragged)
+from pydegensac_b200.matching import (find_absolute_pose_ragged, match_descriptors, match_descriptors_batch,
+                                      match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
+                                      pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
+                                      refine_pose_ragged)
 from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
@@ -51,6 +54,59 @@ def synth_plane(n=1000, seed=1):
     X = np.c_[xy, (6.0 - xy @ nrm[:2]) / nrm[2]]
     x1, x2 = X @ _K.T, (X @ R.T + t) @ _K.T
     return (x1[:, :2] / x1[:, 2:3] + 0.3 * rng.normal(size=(n, 2)), x2[:, :2] / x2[:, 2:3] + 0.3 * rng.normal(size=(n, 2)))
+
+
+def synth_views(n_img=3, n_pts=900, n_clutter=300, D=64, seed=3):
+    """n_img views of one 3-D scene (view i at R_i = rot_y(0.08 i) rot_x(0.02 i), t_i = (0.6, 0.05, 0.1) i, x ~ K (R_i X +
+    t_i)): per view keypoints and descriptors (a shared code per point plus noise, then clutter), and (R_i, t_i)"""
+    rng = np.random.default_rng(seed)
+    X = np.c_[rng.uniform(-4, 4, n_pts), rng.uniform(-4, 4, n_pts), rng.uniform(2, 12, n_pts)]
+    code = rng.normal(size=(n_pts, D)).astype(np.float32)
+    kps, descs, poses = [], [], []
+    for i in range(n_img):
+        R, t = _rot("y", 0.08 * i) @ _rot("x", 0.02 * i), np.array([0.6, 0.05, 0.1]) * i
+        x = (X @ R.T + t) @ _K.T
+        kp = np.r_[x[:, :2] / x[:, 2:3] + 0.1 * rng.normal(size=(n_pts, 2)), rng.uniform(0, 640, (n_clutter, 2))]
+        d = np.r_[code + 0.15 * rng.normal(size=code.shape).astype(np.float32),
+                  rng.normal(size=(n_clutter, D)).astype(np.float32)]
+        perm = rng.permutation(n_pts + n_clutter)
+        kps.append(kp[perm]); descs.append(d[perm]); poses.append((R, t))
+    return kps, descs, poses
+
+
+def register_third_view(dev, K):
+    """Two-view initialisation on views 0 and 1, then view 2 registered against its points, without a host read"""
+    kps, descs, poses = synth_views()
+    kt = [torch.from_numpy(k).to(dev) for k in kps]
+    dt = [torch.from_numpy(d).to(dev) for d in descs]
+    n0 = len(kps[0])
+    m = match_descriptors_batch(dt, [(0, 1)], kt, ratio=0.9, mutual=True)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=[0], offsets=m.offsets,
+                                                    n_max=m.n_max)
+    pose = pose_from_fundamental_ragged(F, K, K, m.pts1, m.pts2, m.offsets, mask)
+    fine = refine_pose_ragged(pose.R, pose.t, K, K, m.pts1, m.pts2, m.offsets, pose.in_front, px_th=1.0)
+    tri = pose_from_fundamental_ragged(fine.F, K, K, m.pts1, m.pts2, m.offsets, fine.inliers)
+    # the points (camera 0's frame, baseline units) onto view 0's keypoints through idx1; slot n0 takes the rows past
+    # the pair's matches, which are never valid
+    live = torch.arange(m.idx1.shape[0], device=dev) < m.offsets[1]
+    slot = torch.where(live, m.idx1, n0)
+    pts0 = torch.full((n0 + 1, 3), float("nan"), dtype=torch.float64, device=dev).index_put_((slot,), tri.points)
+    valid0 = torch.zeros(n0 + 1, dtype=torch.bool, device=dev).index_put_((slot,), tri.in_front & live)
+    # view 2 matched against view 0: its keypoints see view 0's points through idx2
+    m2 = match_descriptors_batch(dt, [(2, 0)], kt, ratio=0.9, mutual=True)
+    live2 = torch.arange(m2.idx2.shape[0], device=dev) < m2.offsets[1]
+    src = torch.where(live2, m2.idx2, n0)
+    view = find_absolute_pose_ragged(m2.pts1, pts0.index_select(0, src), K, m2.offsets,
+                                     valid0.index_select(0, src) & live2, px_th=2.0, seeds=[0])
+    (R0, t0), (R1, t1), (R2, t2) = poses
+    R20 = R2 @ R0.T
+    base = np.linalg.norm(t1 - R1 @ R0.T @ t0)
+    Rv, tv = view.R[0].cpu().numpy(), view.t[0].cpu().numpy()
+    print("view 2 registered: %d inliers after %d RANSAC iterations, MSAC cost %.2f -> %.2f px^2"
+          % (int(view.n_inliers[0]), int(view.iters[0]), float(view.cost0[0]), float(view.cost[0])))
+    print("  rotation error %.2e rad, translation error %.2e baselines (against the planted pose)"
+          % (np.arccos(np.clip((np.trace(Rv @ R20.T) - 1) / 2, -1, 1)),
+             np.linalg.norm(tv - (t2 - R20 @ t0) / base)))
 
 
 def main():
@@ -94,6 +150,7 @@ def main():
               "\nt =", hp.t[0, c].cpu().numpy(), " plane n =", hp.plane[0, c, :3].cpu().numpy(),
               " d = %.3f" % float(hp.plane[0, c, 3]))
     print("median parallax of the chosen pose: %.2f deg" % np.degrees(float(hp.median_angle[0])))
+    register_third_view(dev, K)
 
 
 if __name__ == "__main__":

@@ -405,6 +405,46 @@ int dgb200_refine_fundamental_ragged_dev(const double* d_F, const double* d_x1y1
                                          int max_iters, double px_th, double* d_F_out, double* d_cost0_out,
                                          double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                          uint8_t* d_inliers_out, void* stream);
+/* Absolute pose (registering a view against known 3D points, as cv2.solvePnPRansac) over a RAGGED batch of 2D-3D
+ * correspondences: pair p owns rows d_offsets[p] .. d_offsets[p+1]-1 of d_x [rows][2] (pixels in the view) and
+ * d_X [rows][3] (world points); K [9] row-major, one for all pairs (k_per_pair = 0) or [n_pairs][9]; the pose found
+ * maps x ~ K (R X + t), OpenCV's solvePnP convention.
+ *   Usable rows: d_mask[r] != 0 (every row when d_mask is NULL) and five finite coordinates; n of them, listed in row
+ *   order.  n < 4: no model.  Sampling and scoring see only the list.
+ *   RANSAC: iteration k = 1, 2, ... draws the 3 list entries of the Philox stream's minimal sample of (d_seeds[p], k)
+ *   (csrc/rng.h, as the F / H engines) and solves Lambda Twist P3P (Persson & Nordberg, ECCV 2018) in FP64 on the unit
+ *   bearings normalize(K^-1 [x, y, 1]): 0 to 4 poses, each with positive depths for its three points; a degenerate
+ *   sample gives none and still counts.  A pose's MSAC cost is C = sum over the usable rows of min(e^2, th^2), e^2 the
+ *   squared pixel reprojection error and th = px_th; a row whose depth (R X + t)_z is not positive scores th^2.  A row
+ *   is an inlier when its depth is positive and e^2 <= th^2.  The best pose is replaced only by a strictly lower cost
+ *   (ties keep the earlier iteration and solution).  After iteration k, N_req = min(max_iters, ceil(log(1 - conf) /
+ *   log1p(-w^3))), w = inliers(best) / n (max_iters when conf = 1 or there is no best yet, k when w = 1); iteration
+ *   k + 1 runs only if k < N_req.  The kernel evaluates waves of iterations side by side and applies this rule in
+ *   iteration order, so the result does not depend on the wave width.
+ *   Local optimisation, when the best pose has at least 4 inliers and refine_iters > 0: up to 3 rounds of
+ *   Levenberg-Marquardt on the inliers (two pixel residuals per row, 6 local parameters R <- exp([w]x) R, t <- t + d,
+ *   analytic Jacobian; the schedule of dgb200_refine_pose_ragged_dev with at most refine_iters trial steps, R
+ *   re-orthonormalised when an accepted step left |R R^T - I| above 1e-12), each followed by a re-selection of the
+ *   inliers; it stops when the inlier set does not change (or has fewer than 4 rows).  Its pose replaces the RANSAC
+ *   pose only when its MSAC cost is <= the RANSAC pose's.
+ * The sums of a pair are reduced in a fixed order without atomics: its result does not depend on the batch or the run.
+ * Outputs per pair: d_R_out [9], d_t_out [3] the pose; d_n_inliers_out its inliers; d_iters_out the RANSAC iterations
+ * drawn; d_cost0_out the MSAC cost of the RANSAC pose and d_cost_out that of the output pose (cost <= cost0).
+ * d_mask_out [rows]: 1 for the inliers of the output pose, 0 for every other row of the pair.
+ * Pairs without a model (n < 4, or no sample gave a pose): R = t = 0, n_inliers = 0, iters the iterations drawn, NaN
+ * costs, mask rows 0.  Offsets that decrease, are negative or pass `rows`: the same with iters = 0, no row read or
+ * written.  d_mask may be NULL; d_x, d_X and d_mask_out may be NULL when rows = 0; every other buffer is required.
+ * A null required buffer, n_pairs < 1, rows < 0, px_th not a positive finite number, conf outside (0, 1],
+ * max_iters < 1 or refine_iters < 0 returns DGB200_E_ARG before any launch; the message is
+ * dgb200_absolute_pose_last_error()'s.  Asynchronous on `stream`: one kernel and a stream-ordered workspace of 4 bytes
+ * per row (cudaMallocAsync / cudaFreeAsync), nothing read back. */
+int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, const double* d_K, int k_per_pair,
+                                         const int32_t* d_offsets, int n_pairs, int rows, const uint8_t* d_mask,
+                                         double px_th, double conf, int max_iters, int refine_iters,
+                                         const uint64_t* d_seeds, double* d_R_out, double* d_t_out,
+                                         uint8_t* d_mask_out, int32_t* d_n_inliers_out, int32_t* d_iters_out,
+                                         double* d_cost0_out, double* d_cost_out, void* stream);
+const char* dgb200_absolute_pose_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

@@ -74,6 +74,9 @@ def lib():
                                                           vp]
         L.dgb200_refine_fundamental_ragged_dev.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp, ci, cd, vp, vp, vp, vp, vp,
                                                            vp, vp]
+        L.dgb200_find_absolute_pose_ragged_dev.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, cd, cd, ci, ci, vp, vp, vp,
+                                                           vp, vp, vp, vp, vp, vp]
+        L.dgb200_absolute_pose_last_error.restype = ctypes.c_char_p
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p
         L.dgb200_last_error.restype = ctypes.c_char_p

@@ -44,6 +44,10 @@ matrices), then the guided re-match in the band of the refined F:
 
     fine_f = refine_fundamental_ragged(F, m.pts1, m.pts2, m.offsets, mask, px_th=1.0)
     g = match_descriptors_guided(descs, pairs, kps, fine_f.F, 1.0, guide="F")
+
+A further view registered against the triangulated points (P3P RANSAC on 2D-3D correspondences, cv2.solvePnPRansac):
+
+    view = find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=valid, px_th=2.0)
 """
 import collections
 import ctypes
@@ -60,6 +64,7 @@ RaggedPose = collections.namedtuple("RaggedPose", "R t good points in_front angl
 RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used iters inliers")
 RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_used iters inliers")
 RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost n_used iters inliers")
+AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -537,6 +542,95 @@ def _refine_model_ragged(name, entry, M, pts1, pts2, offsets, mask, max_iters, p
         if rc != 0:
             raise ValueError(L.dgb200_frontend_last_error().decode())
     return Mo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None
+
+
+def find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=None, px_th=2.0, conf=0.999, max_iters=10000, seeds=None,
+                              refine_iters=10):
+    """Register views against known 3D points: P3P MSAC-RANSAC with local optimisation over a ragged batch of 2D-3D
+    correspondences, the batched, device-resident counterpart of cv2.solvePnPRansac.
+
+    All inputs are CUDA tensors on one device: pts2d [rows,2] pixels in the view being registered, pts3d [rows,3]
+    points in the world frame (e.g. the `points` of pose_from_fundamental_ragged, gathered onto the view's matches),
+    K [3,3] or [P,3,3], offsets int32 [P+1] (pair p owns rows offsets[p] .. offsets[p+1]-1), mask [rows] bool / uint8 or
+    None (every row): the rows that may be used (e.g. `in_front`).  Floating inputs are used in float64.  A row is
+    usable when it is in the mask and its five coordinates are finite; a pair needs 4 usable rows.  px_th: the inlier
+    threshold on the reprojection error in pixels (> 0); conf in (0, 1]; max_iters >= 1 bounds the RANSAC iterations;
+    seeds: the seed of each pair's sample stream, as findFundamentalMatrixBatch takes it; refine_iters >= 0 bounds the
+    trial steps of each Levenberg-Marquardt round of the local optimisation (0 skips it).  The estimator, its stopping
+    rule and its local optimisation are specified in include/degensac_b200.h.
+    Returns AbsolutePose(R, t, mask, n_inliers, iters, cost0, cost): R [P,3,3], t [P,3] with x ~ K (R X + t) (OpenCV's
+    solvePnP convention); mask [rows] bool the inliers of the returned pose; n_inliers [P] int32; iters [P] int32 the
+    RANSAC iterations drawn; cost0 [P] the MSAC cost sum min(e^2, px_th^2) of the best RANSAC pose and cost [P] that of
+    the returned pose after local optimisation (cost <= cost0).  A pair without a model (fewer than 4 usable rows, no
+    pose found, malformed offsets) gets R = t = 0, no inliers and NaN costs.  The result of a pair does not depend on
+    the batch it is in.  Asynchronous, nothing is read back."""
+    import torch
+    from .tensor_api import _seeds_tensor
+    named = (("pts2d", pts2d), ("pts3d", pts3d), ("K", K), ("offsets", offsets))
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % nm)
+    if offsets.dim() != 1 or offsets.shape[0] < 2:
+        raise ValueError("offsets must be [P+1] with P >= 1, not %s" % list(offsets.shape))
+    if offsets.dtype != torch.int32:
+        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
+    P = int(offsets.shape[0]) - 1
+    if pts2d.dim() != 2 or pts2d.shape[1] != 2:
+        raise ValueError("pts2d must be [rows,2], not %s" % list(pts2d.shape))
+    rows = int(pts2d.shape[0])
+    if tuple(pts3d.shape) != (rows, 3):
+        raise ValueError("pts3d must be [rows,3] = [%d,3], not %s" % (rows, list(pts3d.shape)))
+    if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
+        raise ValueError("K must be [3,3] or [P,3,3] with P = %d, not %s" % (P, list(K.shape)))
+    for nm, x in (("pts2d", pts2d), ("pts3d", pts3d), ("K", K)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (rows,):
+            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    px_th, conf = float(px_th), float(conf)
+    if not 0.0 < px_th < float("inf"):
+        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
+    if not 0.0 < conf <= 1.0:
+        raise ValueError("conf must lie in (0, 1], not %r" % (conf,))
+    max_iters, refine_iters = int(max_iters), int(refine_iters)
+    if max_iters < 1:
+        raise ValueError("max_iters must be at least 1, not %d" % max_iters)
+    if refine_iters < 0:
+        raise ValueError("refine_iters must not be negative, not %d" % refine_iters)
+    dev = pts2d.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("pts2d, pts3d, K, offsets and mask must be CUDA tensors on one device")
+    if isinstance(seeds, torch.Tensor) and seeds.is_cuda and seeds.device != dev:
+        raise ValueError("seeds must be on the device of pts2d")
+    f64 = torch.float64
+    x, X, Kc = pts2d.to(f64).contiguous(), pts3d.to(f64).contiguous(), K.to(f64).contiguous()
+    off = offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        ds = _seeds_tensor(seeds, P, dev)
+        if tuple(ds.shape) != (P,):
+            raise ValueError("seeds must hold one seed per pair (%d), not %s" % (P, list(ds.shape)))
+        R = torch.empty((P, 3, 3), dtype=f64, device=dev)
+        t = torch.empty((P, 3), dtype=f64, device=dev)
+        mo = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows]
+        n_inl = torch.empty(P, dtype=torch.int32, device=dev)
+        iters = torch.empty(P, dtype=torch.int32, device=dev)
+        cost0 = torch.empty(P, dtype=f64, device=dev)
+        cost = torch.empty(P, dtype=f64, device=dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_find_absolute_pose_ragged_dev(
+            vp(x.data_ptr()), vp(X.data_ptr()), vp(Kc.data_ptr()), int(Kc.dim() == 3), vp(off.data_ptr()), P, rows,
+            vp(m.data_ptr()) if m is not None else None, ctypes.c_double(px_th), ctypes.c_double(conf), max_iters,
+            refine_iters, vp(ds.data_ptr()), vp(R.data_ptr()), vp(t.data_ptr()), vp(mo.data_ptr()),
+            vp(n_inl.data_ptr()), vp(iters.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()),
+            vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_absolute_pose_last_error().decode())
+    return AbsolutePose(R, t, mo.view(torch.bool), n_inl, iters, cost0, cost)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
