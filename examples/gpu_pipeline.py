@@ -10,6 +10,7 @@
     and the H branch for a planar scene:    ->  findHomographyBatch -> pose and scene plane from H
     and a third view:                       ->  its matches to view 0 carry the two-view points (scatter / gather)
                                             ->  absolute pose by P3P RANSAC                (pydegensac_b200.matching)
+                                            ->  3-view tracks triangulated across the registered views
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -28,7 +29,7 @@ import pydegensac_b200 as pydegensac
 from pydegensac_b200.matching import (find_absolute_pose_ragged, match_descriptors, match_descriptors_batch,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
                                       pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
-                                      refine_pose_ragged)
+                                      refine_pose_ragged, triangulate_tracks_ragged)
 from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
@@ -58,11 +59,12 @@ def synth_plane(n=1000, seed=1):
 
 def synth_views(n_img=3, n_pts=900, n_clutter=300, D=64, seed=3):
     """n_img views of one 3-D scene (view i at R_i = rot_y(0.08 i) rot_x(0.02 i), t_i = (0.6, 0.05, 0.1) i, x ~ K (R_i X +
-    t_i)): per view keypoints and descriptors (a shared code per point plus noise, then clutter), and (R_i, t_i)"""
+    t_i)): per view keypoints and descriptors (a shared code per point plus noise, then clutter), (R_i, t_i), the
+    points X and per view the index in X of each keypoint (-1 for clutter)"""
     rng = np.random.default_rng(seed)
     X = np.c_[rng.uniform(-4, 4, n_pts), rng.uniform(-4, 4, n_pts), rng.uniform(2, 12, n_pts)]
     code = rng.normal(size=(n_pts, D)).astype(np.float32)
-    kps, descs, poses = [], [], []
+    kps, descs, poses, ids = [], [], [], []
     for i in range(n_img):
         R, t = _rot("y", 0.08 * i) @ _rot("x", 0.02 * i), np.array([0.6, 0.05, 0.1]) * i
         x = (X @ R.T + t) @ _K.T
@@ -71,12 +73,14 @@ def synth_views(n_img=3, n_pts=900, n_clutter=300, D=64, seed=3):
                   rng.normal(size=(n_clutter, D)).astype(np.float32)]
         perm = rng.permutation(n_pts + n_clutter)
         kps.append(kp[perm]); descs.append(d[perm]); poses.append((R, t))
-    return kps, descs, poses
+        ids.append(np.r_[np.arange(n_pts), np.full(n_clutter, -1)][perm])
+    return kps, descs, poses, X, ids
 
 
 def register_third_view(dev, K):
-    """Two-view initialisation on views 0 and 1, then view 2 registered against its points, without a host read"""
-    kps, descs, poses = synth_views()
+    """Two-view initialisation on views 0 and 1, then view 2 registered against its points and the tracks of view 0's
+    keypoints triangulated across the three views, without a host read"""
+    kps, descs, poses, X, ids = synth_views()
     kt = [torch.from_numpy(k).to(dev) for k in kps]
     dt = [torch.from_numpy(d).to(dev) for d in descs]
     n0 = len(kps[0])
@@ -107,6 +111,28 @@ def register_third_view(dev, K):
     print("  rotation error %.2e rad, translation error %.2e baselines (against the planted pose)"
           % (np.arccos(np.clip((np.trace(Rv @ R20.T) - 1) / 2, -1, 1)),
              np.linalg.norm(tv - (t2 - R20 @ t0) / base)))
+    # 3-slot tracks keyed by view 0's keypoints: the keypoint, its match in view 1 (from the (0, 1) matches) and in
+    # view 2 (from the (2, 0) matches); cameras view 0 = (I, 0), view 1 = the refined pose, view 2 = the registered pose
+    f64 = torch.float64
+    pts = torch.zeros((n0 + 1, 3, 2), dtype=f64, device=dev)
+    seen = torch.zeros((n0 + 1, 3), dtype=torch.bool, device=dev)
+    pts[:n0, 0] = kt[0].to(f64)
+    seen[:n0, 0] = True
+    pts[:, 1].index_put_((slot,), m.pts2.to(f64))
+    seen[:, 1].index_put_((slot,), live)
+    pts[:, 2].index_put_((src,), m2.pts1.to(f64))
+    seen[:, 2].index_put_((src,), live2)
+    R = torch.stack([torch.eye(3, dtype=f64, device=dev), fine.R[0], view.R[0]])
+    t = torch.stack([torch.zeros(3, dtype=f64, device=dev), fine.t[0], view.t[0]])
+    cams = torch.arange(3, dtype=torch.int32, device=dev).repeat(n0)
+    offsets = torch.arange(0, 3 * n0 + 1, 3, dtype=torch.int32, device=dev)
+    tr = triangulate_tracks_ragged(cams, pts[:n0].reshape(-1, 2), R, t, K, offsets, seen[:n0].reshape(-1), px_th=2.0)
+    n_in = tr.n_inliers.cpu().numpy()
+    ok = (n_in >= 2) & (ids[0] >= 0)
+    truth = (X[ids[0][ok]] @ R0.T + t0) / base                # the planted points in camera 0's frame, baseline units
+    err = np.linalg.norm(tr.X.cpu().numpy()[ok] - truth, axis=1)
+    print("tracks of view 0's %d keypoints: %d triangulated (%d from all three views), median 3D error %.2e baselines "
+          "against the planted points" % (n0, int((n_in >= 2).sum()), int((n_in == 3).sum()), float(np.median(err))))
 
 
 def main():

@@ -445,6 +445,58 @@ int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, c
                                          uint8_t* d_mask_out, int32_t* d_n_inliers_out, int32_t* d_iters_out,
                                          double* d_cost0_out, double* d_cost_out, void* stream);
 const char* dgb200_absolute_pose_last_error(void);
+/* Triangulation of tracks across registered views (the step after registering a view in an incremental
+ * reconstruction) over a RAGGED batch of tracks: track j owns observations d_offsets[j] .. d_offsets[j+1]-1, each a
+ * camera index d_cams [obs] and a pixel d_pts [obs][2].  Camera c has the pose d_R [n_cams][9] (row-major),
+ * d_t [n_cams][3], world to camera, so that x ~ K (R X + t) (the convention of dgb200_find_absolute_pose_ragged_dev's
+ * output), and K [9], one for all cameras (k_per_camera = 0) or [n_cams][9].  All arithmetic is FP64.
+ *   Usable observations: d_mask[r] != 0 (every row when d_mask is NULL), 0 <= d_cams[r] < n_cams, two finite pixel
+ *   coordinates, and a registered camera: the 12 entries of (R, t) finite and det R > 0.5 (this rejects the R = t = 0
+ *   of a view that could not be registered).  n of them, listed in row order.  n < 2: no model.
+ *   World rays: centre C = -R^T t and direction d = R^T normalize(K^-1 [x, y, 1]).
+ *   Hypothesis of list entries (i, j): none when both come from one camera; otherwise b = d_i . d_j, w = C_i - C_j,
+ *   none when b > cos(min_angle) or 1 - b^2 <= 0 (the triangulation-angle gate, which also rejects parallel rays);
+ *   lambda_i = (b (d_j . w) - d_i . w) / (1 - b^2), lambda_j = (d_j . w - b (d_i . w)) / (1 - b^2), none unless both
+ *   are > 0; X = ((C_i + lambda_i d_i) + (C_j + lambda_j d_j)) / 2, the midpoint of the common perpendicular (+, -, x,
+ *   / and sqrt only, with dots summed left to right, so that every build gives the same bits).  A missing hypothesis
+ *   still counts as an iteration.
+ *   Iterations: M = n (n - 1) / 2 pairs and K_max = min(M, max_iters).  When M <= max_iters, iteration k = 1, 2, ...
+ *   is the k-th pair (i < j) in lexicographic order, (0, 1), (0, 2), ..., (1, 2), ...: short tracks are enumerated
+ *   exhaustively and deterministically.  Otherwise iteration k is (i, j) = the Philox stream's minimal sample of 2 of
+ *   (d_seeds[j], k) (csrc/rng.h, as the F / H / P3P engines), in draw order.
+ *   Score: the MSAC cost sum over the usable observations of min(e^2, th^2), e^2 the squared pixel reprojection error
+ *   in the observation's camera and th = px_th; an observation with depth (R X + t)_z <= 0 scores th^2.  It is an
+ *   inlier when its depth is > 0 and e^2 <= th^2.  The best point is replaced only by a strictly lower cost.  After
+ *   iteration k, N_req = min(K_max, ceil(log(1 - conf) / log1p(-w^2))), w = inliers(best) / n (K_max when conf = 1 or
+ *   there is no best yet, k when w = 1); iteration k + 1 runs only if k < N_req.  The kernel evaluates waves of 32
+ *   iterations side by side and applies this rule in iteration order, so the result does not depend on the wave width.
+ *   Local optimisation, when the best point has at least 2 inliers and refine_iters > 0: up to 3 rounds of
+ *   Levenberg-Marquardt on the inliers' pixel residuals over X (X <- X + D, analytic Jacobian; the schedule of
+ *   dgb200_refine_pose_ragged_dev with at most refine_iters trial steps), each followed by a re-selection of the
+ *   inliers; it stops when the inlier set does not change (or has fewer than 2 rows).  Its point replaces the RANSAC
+ *   point only when its MSAC cost is <= the RANSAC point's.
+ * A track is one warp and its sums are reduced in a fixed order without atomics: its result does not depend on the
+ * batch or the run.  Outputs per track: d_X_out [3] the point; d_n_inliers_out its inliers; d_iters_out the
+ * hypotheses drawn or enumerated; d_cost0_out the MSAC cost of the RANSAC point and d_cost_out that of the output point
+ * (cost <= cost0); d_angle_out the largest triangulation angle at X, atan2(|a x b|, a . b) with a = X - C_i and
+ * b = X - C_j, over pairs of inliers from distinct cameras (0 without such a pair; the caller applies its threshold).
+ * d_mask_out [obs]: 1 for the inliers of the output point, 0 for every other row of the track.
+ * Tracks without a model (n < 2, or no hypothesis: one camera only, every angle too small, every pair behind a
+ * centre): X = NaN, n_inliers = 0, iters the iterations run, NaN costs and angle, mask rows 0.  Offsets that decrease,
+ * are negative or pass `obs`: the same with iters = 0, no row read or written.  d_mask may be NULL; d_cams, d_pts and
+ * d_mask_out may be NULL when obs = 0; every other buffer is required.  A null required buffer, n_tracks < 1, obs < 0,
+ * n_cams < 1, px_th not a positive finite number, min_angle outside [0, pi), conf outside (0, 1], max_iters < 1 or
+ * refine_iters < 0 returns DGB200_E_ARG before any launch; the message is dgb200_triangulate_last_error()'s.
+ * Asynchronous on `stream`: two kernels (the camera table, then the tracks) and a stream-ordered workspace of
+ * 272 bytes per camera and 4 bytes per observation (cudaMallocAsync / cudaFreeAsync), nothing read back. */
+int dgb200_triangulate_tracks_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R,
+                                         const double* d_t, const double* d_K, int k_per_camera, int n_cams,
+                                         const int32_t* d_offsets, int n_tracks, int obs, const uint8_t* d_mask,
+                                         double px_th, double min_angle, double conf, int max_iters, int refine_iters,
+                                         const uint64_t* d_seeds, double* d_X_out, uint8_t* d_mask_out,
+                                         int32_t* d_n_inliers_out, int32_t* d_iters_out, double* d_cost0_out,
+                                         double* d_cost_out, double* d_angle_out, void* stream);
+const char* dgb200_triangulate_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

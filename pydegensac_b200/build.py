@@ -33,10 +33,11 @@ def build_cuda(force=False, verbose=False):
     src = os.path.join(CSRC, "degensac_b200.cu")
     src2 = os.path.join(CSRC, "frontend.cu")      # matcher / pose / QR null space (the steps either side of the path)
     src3 = os.path.join(CSRC, "absolute_pose.cu")  # P3P RANSAC: registering a view against known 3D points
+    src4 = os.path.join(CSRC, "triangulate.cu")    # multi-view triangulation of tracks across registered views
     if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest(_csrc_files()):
         return LIB
     nvcc = os.environ.get("NVCC", "nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3]
+    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3, src4]
     subprocess.check_call(cmd)
     return LIB
 

@@ -135,15 +135,26 @@ DG_HD void ap_step(const double* P, const double* D, double* P2) {
   for (int i = 0; i < 3; ++i) P2[9 + i] = P[9 + i] + D[3 + i];
 }
 
-// The iterations the sequential rule requires after an iteration k whose best pose has `inl` of n inliers:
-// min(max_iters, ceil(log(1 - conf) / log1p(-w^3))), w = inl / n; max_iters when conf == 1 or there is no best pose
-// yet (has_best false), k when w == 1.
-DG_HD int ap_required_iters(bool has_best, int inl, int n, double conf, int max_iters, int k) {
+// w^S as ((w w) w) ...
+template <int S>
+DG_HD double ipow(double w) {
+  if constexpr (S == 1) return w;
+  else return ipow<S - 1>(w) * w;
+}
+
+// The iterations the sequential rule requires after an iteration k whose best model, fitted to samples of S rows, has
+// `inl` of n inliers: min(max_iters, ceil(log(1 - conf) / log1p(-w^S))), w = inl / n; max_iters when conf == 1 or
+// there is no best model yet (has_best false), k when w == 1.
+template <int S>
+DG_HD int required_iters(bool has_best, int inl, int n, double conf, int max_iters, int k) {
   if (!has_best || conf >= 1.0) return max_iters;
   if (inl >= n) return k;
   const double w = (double)inl / (double)n;
-  const double q = ceil(log(1.0 - conf) / log1p(-(w * w * w)));
+  const double q = ceil(log(1.0 - conf) / log1p(-ipow<S>(w)));
   return q < (double)max_iters ? (int)q : max_iters;
+}
+DG_HD int ap_required_iters(bool has_best, int inl, int n, double conf, int max_iters, int k) {
+  return required_iters<3>(has_best, inl, n, conf, max_iters, k);
 }
 
 }  // namespace dg

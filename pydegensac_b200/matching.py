@@ -48,9 +48,14 @@ matrices), then the guided re-match in the band of the refined F:
 A further view registered against the triangulated points (P3P RANSAC on 2D-3D correspondences, cv2.solvePnPRansac):
 
     view = find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=valid, px_th=2.0)
+
+Tracks triangulated across the registered views (two-ray midpoint RANSAC with local optimisation on each track):
+
+    tr = triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=observed, px_th=2.0)
 """
 import collections
 import ctypes
+import math
 
 import numpy as np
 
@@ -65,6 +70,7 @@ RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used ite
 RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_used iters inliers")
 RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost n_used iters inliers")
 AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
+Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -631,6 +637,106 @@ def find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=None, px_th=2.0, co
         if rc != 0:
             raise ValueError(L.dgb200_absolute_pose_last_error().decode())
     return AbsolutePose(R, t, mo.view(torch.bool), n_inl, iters, cost0, cost)
+
+
+def triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=None, px_th=2.0, min_angle=math.radians(1.5),
+                              conf=0.999, max_iters=1000, seeds=None, refine_iters=10):
+    """Triangulate tracks across registered views: two-ray midpoint MSAC-RANSAC with local optimisation over a ragged
+    batch of tracks, each a list of observations (camera index, pixel) of one scene point.
+
+    All inputs are CUDA tensors on one device: cams int32 [obs] the camera of each observation, pts [obs,2] its pixel,
+    R [C,3,3] and t [C,3] the cameras' poses, world to camera with x ~ K (R X + t) (what find_absolute_pose_ragged
+    returns; a camera whose R, t are not finite or whose det R <= 0.5, such as the R = t = 0 of a view that was not
+    registered, is skipped), K [3,3] or [C,3,3], offsets int32 [T+1] (track j owns observations offsets[j] ..
+    offsets[j+1]-1), mask [obs] bool / uint8 or None (every row): the observations that may be used.  A fixed-width
+    layout (one slot per view, mask = observed) is a valid input.  Floating inputs are used in float64.  px_th: the
+    inlier threshold on the reprojection error in pixels (> 0); min_angle in [0, pi): the smallest angle between the
+    two rays of a hypothesis, in radians; conf in (0, 1]; max_iters >= 1 bounds the hypotheses per track (a track
+    whose pairs are no more than max_iters tries every pair, in order); seeds: the seed of each track's sample stream,
+    as findFundamentalMatrixBatch takes it; refine_iters >= 0 bounds the trial steps of each Levenberg-Marquardt round
+    of the local optimisation (0 skips it).  The estimator is specified in include/degensac_b200.h.
+    Returns Tracks(X, mask, n_inliers, iters, cost0, cost, angle): X [T,3] the points in the world frame; mask [obs]
+    bool the inliers of the returned point; n_inliers [T] int32; iters [T] int32 the hypotheses drawn or enumerated;
+    cost0 [T] the MSAC cost sum min(e^2, px_th^2) of the best RANSAC point and cost [T] that of the returned point
+    (cost <= cost0); angle [T] the largest triangulation angle at X over pairs of inliers from distinct cameras, in
+    radians (0 without such a pair; filter on it as COLMAP does).  A track without a model (fewer than 2 usable
+    observations, no hypothesis, malformed offsets) gets X = NaN, no inliers and NaN costs and angle.  The result of a
+    track does not depend on the batch it is in.  Asynchronous, nothing is read back."""
+    import torch
+    from .tensor_api import _seeds_tensor
+    named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("K", K), ("offsets", offsets))
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % nm)
+    if offsets.dim() != 1 or offsets.shape[0] < 2:
+        raise ValueError("offsets must be [T+1] with T >= 1, not %s" % list(offsets.shape))
+    for nm, x in (("offsets", offsets), ("cams", cams)):
+        if x.dtype != torch.int32:
+            raise ValueError("%s must be int32, not %s" % (nm, x.dtype))
+    T = int(offsets.shape[0]) - 1
+    if pts.dim() != 2 or pts.shape[1] != 2:
+        raise ValueError("pts must be [obs,2], not %s" % list(pts.shape))
+    obs = int(pts.shape[0])
+    if tuple(cams.shape) != (obs,):
+        raise ValueError("cams must be [obs] = [%d], not %s" % (obs, list(cams.shape)))
+    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
+        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
+    C = int(R.shape[0])
+    if tuple(t.shape) != (C, 3):
+        raise ValueError("t must be [C,3] = [%d,3], not %s" % (C, list(t.shape)))
+    if tuple(K.shape) not in ((3, 3), (C, 3, 3)):
+        raise ValueError("K must be [3,3] or [C,3,3] with C = %d, not %s" % (C, list(K.shape)))
+    for nm, x in (("pts", pts), ("R", R), ("t", t), ("K", K)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (obs,):
+            raise ValueError("mask must be [obs] = [%d], not %s" % (obs, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    px_th, min_angle, conf = float(px_th), float(min_angle), float(conf)
+    if not 0.0 < px_th < float("inf"):
+        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
+    if not 0.0 <= min_angle < math.pi:
+        raise ValueError("min_angle must lie in [0, pi), not %r" % (min_angle,))
+    if not 0.0 < conf <= 1.0:
+        raise ValueError("conf must lie in (0, 1], not %r" % (conf,))
+    max_iters, refine_iters = int(max_iters), int(refine_iters)
+    if max_iters < 1:
+        raise ValueError("max_iters must be at least 1, not %d" % max_iters)
+    if refine_iters < 0:
+        raise ValueError("refine_iters must not be negative, not %d" % refine_iters)
+    dev = pts.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("cams, pts, R, t, K, offsets and mask must be CUDA tensors on one device")
+    if isinstance(seeds, torch.Tensor) and seeds.is_cuda and seeds.device != dev:
+        raise ValueError("seeds must be on the device of pts")
+    f64 = torch.float64
+    x, Rc, tc, Kc = (v.to(f64).contiguous() for v in (pts, R, t, K))
+    cm, off = cams.contiguous(), offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        ds = _seeds_tensor(seeds, T, dev)
+        if tuple(ds.shape) != (T,):
+            raise ValueError("seeds must hold one seed per track (%d), not %s" % (T, list(ds.shape)))
+        X = torch.empty((T, 3), dtype=f64, device=dev)
+        mo = torch.empty(max(obs, 1), dtype=torch.uint8, device=dev)[:obs]
+        n_inl = torch.empty(T, dtype=torch.int32, device=dev)
+        iters = torch.empty(T, dtype=torch.int32, device=dev)
+        cost0 = torch.empty(T, dtype=f64, device=dev)
+        cost = torch.empty(T, dtype=f64, device=dev)
+        angle = torch.empty(T, dtype=f64, device=dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_triangulate_tracks_ragged_dev(
+            vp(cm.data_ptr()), vp(x.data_ptr()), vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(Kc.data_ptr()),
+            int(Kc.dim() == 3), C, vp(off.data_ptr()), T, obs, vp(m.data_ptr()) if m is not None else None,
+            ctypes.c_double(px_th), ctypes.c_double(min_angle), ctypes.c_double(conf), max_iters, refine_iters,
+            vp(ds.data_ptr()), vp(X.data_ptr()), vp(mo.data_ptr()), vp(n_inl.data_ptr()), vp(iters.data_ptr()),
+            vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(angle.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_triangulate_last_error().decode())
+    return Tracks(X, mo.view(torch.bool), n_inl, iters, cost0, cost, angle)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
