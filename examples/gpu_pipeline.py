@@ -11,6 +11,7 @@
     and a third view:                       ->  its matches to view 0 carry the two-view points (scatter / gather)
                                             ->  absolute pose by P3P RANSAC                (pydegensac_b200.matching)
                                             ->  3-view tracks triangulated across the registered views
+                                            ->  views 1 and 2 and the tracks bundle-adjusted, view 0 held
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -29,7 +30,7 @@ import pydegensac_b200 as pydegensac
 from pydegensac_b200.matching import (find_absolute_pose_ragged, match_descriptors, match_descriptors_batch,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
                                       pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
-                                      refine_pose_ragged, triangulate_tracks_ragged)
+                                      refine_pose_ragged, triangulate_tracks_ragged, bundle_adjust_ragged)
 from pydegensac_b200.scenes import scene_F, _K, _rot
 
 
@@ -133,6 +134,20 @@ def register_third_view(dev, K):
     err = np.linalg.norm(tr.X.cpu().numpy()[ok] - truth, axis=1)
     print("tracks of view 0's %d keypoints: %d triangulated (%d from all three views), median 3D error %.2e baselines "
           "against the planted points" % (n0, int((n_in >= 2).sum()), int((n_in == 3).sum()), float(np.median(err))))
+    # bundle adjustment: views 1 and 2 and every track's point refined jointly, view 0 held and one translation
+    # coordinate of view 1 held (the scale)
+    ba = bundle_adjust_ragged(cams, pts[:n0].reshape(-1, 2), R, t, K, offsets, tr.X, mask=tr.mask, free=[1, 2],
+                              scale_gauge=1, loss_scale=1.0)
+    Rp = [R1 @ R0.T, R20]
+
+    def rot_err(Rs):
+        return sum(np.arccos(np.clip((np.trace(Rs[c].cpu().numpy() @ Rp[c - 1].T) - 1) / 2, -1, 1)) for c in (1, 2))
+    # (the planted points are in baseline units: the adjusted scene is scaled back to |t_1| = 1 first)
+    err_ba = np.linalg.norm(ba.X.cpu().numpy()[ok] / np.linalg.norm(ba.t[1].cpu().numpy()) - truth, axis=1)
+    print("bundle adjustment of views 1 and 2 over %d observations in %d trial steps: cost %.2f -> %.2f" %
+          (int(ba.n_used[0]), int(ba.iters[0]), float(ba.cost0[0]), float(ba.cost[0])))
+    print("  summed rotation error of views 1 and 2 %.2e -> %.2e rad, median 3D error %.2e -> %.2e baselines"
+          % (rot_err(R), rot_err(ba.R), float(np.median(err)), float(np.median(err_ba))))
 
 
 def main():

@@ -497,6 +497,58 @@ int dgb200_triangulate_tracks_ragged_dev(const int32_t* d_cams, const double* d_
                                          int32_t* d_n_inliers_out, int32_t* d_iters_out, double* d_cost0_out,
                                          double* d_cost_out, double* d_angle_out, void* stream);
 const char* dgb200_triangulate_last_error(void);
+/* Bundle adjustment of registered views and their tracks (the step after registering a view and triangulating its
+ * tracks in an incremental reconstruction): Levenberg-Marquardt over the free cameras' poses and the tracks' points
+ * jointly.  Tracks and cameras have the layout and convention of dgb200_triangulate_tracks_ragged_dev: track j owns
+ * observations d_offsets[j] .. d_offsets[j+1]-1 (camera d_cams [obs], pixel d_pts [obs][2]), camera c has d_R [9],
+ * d_t [3] with x ~ K (R X + t) and K [9] (k_per_camera as there); d_X [n_tracks][3] are the tracks' points (the output
+ * of the triangulation).  All arithmetic is FP64; the intrinsics are held.
+ *   Free and held cameras: h_free [n_free] is a HOST list of 0 to 64 distinct camera indices, copied into the kernels'
+ *   parameter block; every other camera is held (its observations constrain the points, its pose does not move).
+ *   Usable observations: d_mask[r] != 0 (every row when d_mask is NULL), 0 <= d_cams[r] < n_cams, a registered camera
+ *   (the 12 entries of (R, t) finite and det R > 0.5), a finite pixel, a finite X of its track and depth (R X + t)_z > 0
+ *   at the start.  A track is optimised when its usable observations come from at least 2 distinct cameras and V_p =
+ *   sum w J_X^T J_X over them has a positive Cholesky factor at the start; its usable observations are then used.  Any
+ *   other track's X is copied bit for bit and its observations are not used.  A free camera without a used observation
+ *   is held and passed through.
+ *   Scale gauge: scale_gauge = -1, or a camera g of h_free when a camera outside h_free exists.  With a = the lowest
+ *   index outside h_free and c_a = -R_a^T t_a, translation coordinate argmax |t_g + R_g c_a| of g is held (the lower
+ *   axis on ties; chosen on the device from the input poses): g's translation relative to a keeps its scale.
+ *   Cost C = sum over the used observations of rho(e^2), e^2 the squared pixel reprojection error: rho(s) = s when
+ *   loss_scale = 0, else the Cauchy loss sigma^2 log(1 + s / sigma^2) with sigma = loss_scale.  The normal equations
+ *   use the IRLS weights w = rho'(e^2) at the linearisation point (no second-order correction).
+ *   Parameters: per free camera 6, R <- exp([w]x) R, t <- t + d (the update of the P3P local optimisation), the held
+ *   coordinate dropped; per optimised track 3, X <- X + D.  A trial R whose |R R^T - I| exceeds 1e-12 is
+ *   re-orthonormalised before it is scored, so the output's cost is the cost reported.
+ *   Trial step: U*_a = U_a + lambda diag U_a, V*_p = V_p + lambda diag V_p; the reduced camera system S dc = -(g_c -
+ *   sum_p W_p V*_p^-1 g_p), S = U* - sum_p W_p V*_p^-1 W_p^T, is solved by a dense FP64 Cholesky (rows of held
+ *   coordinates and of cameras without used observations replaced by identity rows with a zero right-hand side);
+ *   dX_p = -V*_p^-1 (g_p + sum_i W_i^T dc_cam(i)).  A non-positive pivot of S or of any V*_p rejects the step, and a
+ *   used observation with depth <= 0 at the trial point costs +inf.
+ *   Schedule, that of dgb200_refine_pose_ragged_dev: lambda starts at 1e-3; a strictly lower cost accepts the step
+ *   and sets lambda <- max(lambda / 10, 1e-12), otherwise lambda <- 10 lambda; it stops after max_iters trial steps,
+ *   after a trial step that changes the cost by less than 1e-12 of it, or when lambda > 1e8.
+ * Every sum is reduced in a fixed order without atomics: a rerun gives the same bytes.  Outputs: d_R_out [n_cams][9],
+ * d_t_out [n_cams][3] (held cameras bit-identical to the input), d_X_out [n_tracks][3] (tracks that were not optimised
+ * bit-identical), d_mask_out [obs]: 1 for a usable observation with depth > 0 and e^2 <= px_th^2 at the output, 0 for
+ * every other row; d_cost0_out [1] and d_cost_out [1] the cost at the start and at the output (cost <= cost0);
+ * d_iters_out [1] the trial steps taken; d_n_used_out [1] the used observations.  Output buffers may alias the
+ * inputs.  A track with offsets that decrease, are negative or pass `obs` is not optimised and none of its rows is
+ * read.  d_mask may be NULL; d_cams, d_pts and d_mask_out may be NULL when obs = 0.  A null required buffer,
+ * n_tracks < 1, obs < 0, n_cams < 1, n_free outside [0, 64], a repeated or out-of-range index in h_free, a scale_gauge
+ * that is neither -1 nor in h_free (or with no camera outside h_free), a loss_scale that is neither 0 nor a positive
+ * finite number, max_iters < 0 or px_th not a positive finite number returns DGB200_E_ARG before any launch; the
+ * message is dgb200_bundle_adjust_last_error()'s.  Asynchronous on `stream`: 6 kernels per trial step and 7 around
+ * them, and a stream-ordered workspace (cudaMallocAsync / cudaFreeAsync) of 418 bytes per observation, 180 bytes per
+ * track, 468 bytes per camera and 8 (6 n_free)^2 bytes for S; nothing read back. */
+int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R, const double* d_t,
+                                    const double* d_K, int k_per_camera, int n_cams, const int32_t* d_offsets,
+                                    int n_tracks, int obs, const double* d_X, const uint8_t* d_mask,
+                                    const int32_t* h_free, int n_free, int scale_gauge, double loss_scale,
+                                    int max_iters, double px_th, double* d_R_out, double* d_t_out, double* d_X_out,
+                                    uint8_t* d_mask_out, double* d_cost0_out, double* d_cost_out,
+                                    int32_t* d_iters_out, int32_t* d_n_used_out, void* stream);
+const char* dgb200_bundle_adjust_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

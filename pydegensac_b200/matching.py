@@ -52,6 +52,10 @@ A further view registered against the triangulated points (P3P RANSAC on 2D-3D c
 Tracks triangulated across the registered views (two-ray midpoint RANSAC with local optimisation on each track):
 
     tr = triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=observed, px_th=2.0)
+
+Cameras and points refined jointly (bundle adjustment, Levenberg-Marquardt with the Schur complement), view 0 held:
+
+    ba = bundle_adjust_ragged(cams, pts, R, t, K, offsets, tr.X, mask=tr.mask, free=[1, 2], scale_gauge=1)
 """
 import collections
 import ctypes
@@ -71,6 +75,7 @@ RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_
 RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost n_used iters inliers")
 AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
 Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
+BundleAdjustment = collections.namedtuple("BundleAdjustment", "R t X mask cost0 cost iters n_used")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -737,6 +742,135 @@ def triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=None, px_th=2.0,
         if rc != 0:
             raise ValueError(L.dgb200_triangulate_last_error().decode())
     return Tracks(X, mo.view(torch.bool), n_inl, iters, cost0, cost, angle)
+
+
+BA_MAX_FREE = 64   # free cameras per call at most (the reduced camera system is dense)
+
+
+def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, scale_gauge="auto", loss_scale=None,
+                         max_iters=50, px_th=2.0):
+    """Bundle-adjust registered views and their tracks: Levenberg-Marquardt over the free cameras' poses and the
+    tracks' points jointly, the points eliminated by the Schur complement and the reduced camera system solved densely.
+
+    cams, pts, R, t, K, offsets and mask are CUDA tensors on one device, laid out as triangulate_tracks_ragged takes
+    them (x ~ K (R X + t); a camera whose R, t are not finite or whose det R <= 0.5 is not registered, and its
+    observations are not used).  X [T,3] the tracks' points and mask [obs] (bool / uint8 or None: every row) the
+    observations that may be used: the X and mask of triangulate_tracks_ragged feed straight in.  Floating inputs are
+    used in float64; the intrinsics are held.
+    free: a HOST sequence of at most 64 distinct camera indices whose poses move (control data, as match_descriptors_
+    batch's pairs); every other camera is held.  None: every camera but camera 0, a ValueError when that is more than
+    64.  scale_gauge: a camera of `free` one of whose translation coordinates is held, which fixes the scale that one
+    held camera leaves free (the axis of its largest translation relative to the lowest-index held camera, chosen on
+    the device); "auto": free[0] when exactly one camera is held, else None; None: no scale hold.  loss_scale: None for
+    the squared pixel error, sigma > 0 for the Cauchy loss sigma^2 log(1 + e^2 / sigma^2).  max_iters >= 0 bounds the
+    trial steps.  px_th > 0: the inlier threshold of the output mask, in pixels.  The estimator is specified in
+    include/degensac_b200.h.
+    Returns BundleAdjustment(R, t, X, mask, cost0, cost, iters, n_used): R [C,3,3], t [C,3] and X [T,3] (held cameras
+    and tracks that were not optimised -- fewer than 2 distinct cameras, or a point behind all but one -- bit-identical
+    to the input); mask [obs] bool: the usable observations with positive depth and a reprojection error <= px_th at
+    the output; cost0, cost: [1] float64 the cost at the start and at the output (cost <= cost0); iters: [1] int32 the
+    trial steps; n_used: [1] int32 the observations in the cost.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("K", K), ("offsets", offsets), ("X", X))
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % nm)
+    if offsets.dim() != 1 or offsets.shape[0] < 2:
+        raise ValueError("offsets must be [T+1] with T >= 1, not %s" % list(offsets.shape))
+    for nm, x in (("offsets", offsets), ("cams", cams)):
+        if x.dtype != torch.int32:
+            raise ValueError("%s must be int32, not %s" % (nm, x.dtype))
+    T = int(offsets.shape[0]) - 1
+    if pts.dim() != 2 or pts.shape[1] != 2:
+        raise ValueError("pts must be [obs,2], not %s" % list(pts.shape))
+    obs = int(pts.shape[0])
+    if tuple(cams.shape) != (obs,):
+        raise ValueError("cams must be [obs] = [%d], not %s" % (obs, list(cams.shape)))
+    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
+        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
+    C = int(R.shape[0])
+    if tuple(t.shape) != (C, 3):
+        raise ValueError("t must be [C,3] = [%d,3], not %s" % (C, list(t.shape)))
+    if tuple(K.shape) not in ((3, 3), (C, 3, 3)):
+        raise ValueError("K must be [3,3] or [C,3,3] with C = %d, not %s" % (C, list(K.shape)))
+    if tuple(X.shape) != (T, 3):
+        raise ValueError("X must be [T,3] = [%d,3], not %s" % (T, list(X.shape)))
+    for nm, x in (("pts", pts), ("R", R), ("t", t), ("K", K), ("X", X)):
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
+    if mask is not None:
+        if tuple(mask.shape) != (obs,):
+            raise ValueError("mask must be [obs] = [%d], not %s" % (obs, list(mask.shape)))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    if free is None:
+        if C - 1 > BA_MAX_FREE:
+            raise ValueError("free=None frees %d cameras, more than %d: pass an explicit free list" % (C - 1, BA_MAX_FREE))
+        free = list(range(1, C))
+    free = _host_pairs(free)
+    try:
+        fr = [int(c) for c in np.asarray(free).reshape(-1)]
+    except (TypeError, ValueError):
+        raise ValueError("free must be a host sequence of camera indices")
+    if len(fr) > BA_MAX_FREE:
+        raise ValueError("free holds %d cameras, more than %d" % (len(fr), BA_MAX_FREE))
+    if len(set(fr)) != len(fr):
+        raise ValueError("free holds a camera twice")
+    if any(not 0 <= c < C for c in fr):
+        raise ValueError("free holds a camera index outside [0, %d)" % C)
+    n_held = C - len(fr)
+    if isinstance(scale_gauge, str):
+        if scale_gauge != "auto":
+            raise ValueError("scale_gauge must be 'auto', None or a camera of free, not %r" % (scale_gauge,))
+        gauge = fr[0] if n_held == 1 and fr else -1
+    elif scale_gauge is None:
+        gauge = -1
+    else:
+        gauge = int(scale_gauge)
+        if gauge not in fr:
+            raise ValueError("scale_gauge %d is not one of the free cameras" % gauge)
+        if n_held == 0:
+            raise ValueError("scale_gauge needs a held camera: every camera is free")
+    if loss_scale is None:
+        sigma = 0.0
+    else:
+        sigma = float(loss_scale)
+        if not 0.0 < sigma < float("inf"):
+            raise ValueError("loss_scale must be a positive number or None, not %r" % (loss_scale,))
+    max_iters, px_th = int(max_iters), float(px_th)
+    if max_iters < 0:
+        raise ValueError("max_iters must not be negative, not %d" % max_iters)
+    if not 0.0 < px_th < float("inf"):
+        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
+    dev = pts.device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("cams, pts, R, t, K, offsets, X and mask must be CUDA tensors on one device")
+    f64 = torch.float64
+    x, Rc, tc, Kc, Xc = (v.to(f64).contiguous() for v in (pts, R, t, K, X))
+    cm, off = cams.contiguous(), offsets.contiguous()
+    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    hf = np.ascontiguousarray(fr, dtype=np.int32)
+    L = _cabi.lib()
+    with torch.cuda.device(dev):
+        Ro = torch.empty((C, 3, 3), dtype=f64, device=dev)
+        to = torch.empty((C, 3), dtype=f64, device=dev)
+        Xo = torch.empty((T, 3), dtype=f64, device=dev)
+        mo = torch.empty(max(obs, 1), dtype=torch.uint8, device=dev)[:obs]
+        cost0 = torch.empty(1, dtype=f64, device=dev)
+        cost = torch.empty(1, dtype=f64, device=dev)
+        iters = torch.empty(1, dtype=torch.int32, device=dev)
+        n_used = torch.empty(1, dtype=torch.int32, device=dev)
+        vp = ctypes.c_void_p
+        rc = L.dgb200_bundle_adjust_ragged_dev(
+            vp(cm.data_ptr()), vp(x.data_ptr()), vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(Kc.data_ptr()),
+            int(Kc.dim() == 3), C, vp(off.data_ptr()), T, obs, vp(Xc.data_ptr()),
+            vp(m.data_ptr()) if m is not None else None, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr),
+            gauge, ctypes.c_double(sigma), max_iters, ctypes.c_double(px_th), vp(Ro.data_ptr()), vp(to.data_ptr()),
+            vp(Xo.data_ptr()), vp(mo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(iters.data_ptr()),
+            vp(n_used.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
+        if rc != 0:
+            raise ValueError(L.dgb200_bundle_adjust_last_error().decode())
+    return BundleAdjustment(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
