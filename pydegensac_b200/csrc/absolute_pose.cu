@@ -20,30 +20,20 @@
 #include <stdio.h>
 
 #include "../../include/degensac_b200.h"
+#include "entry_error.h"
 #include "common.h"
 #include "rng.h"
 #include "p3p.h"
 #include "absolute_pose.h"
+#include "device_util.h"
 
 namespace {
 
-thread_local char g_err3[256] = "";
-int fail3(int code, const char* what, cudaError_t e = cudaSuccess) {
-  if (e != cudaSuccess) snprintf(g_err3, sizeof(g_err3), "%s: %s", what, cudaGetErrorString(e));
-  else snprintf(g_err3, sizeof(g_err3), "%s", what);
-  return code;
-}
-#define CU3(call)                                                     \
-  do {                                                                \
-    cudaError_t e__ = (call);                                         \
-    if (e__ != cudaSuccess) return fail3(DGB200_E_CUDA, #call, e__);  \
-  } while (0)
+thread_local char g_err[256] = "";
+int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_error(g_err, code, what, e); }
 
 constexpr int kApThreads = 128;
 constexpr int kApWarps = kApThreads / 32;     // the wave width: iterations evaluated side by side
-
-__device__ __forceinline__ double qnan3() { return __longlong_as_double(0x7ff8000000000000ll); }
-__device__ __forceinline__ bool finite3(double v) { return fabs(v) < INFINITY; }
 
 struct AbsPoseArgs {
   const double* x; const double* X; const double* K;      // [rows][2], [rows][3]; K [9] shared or [P][9]
@@ -196,8 +186,8 @@ __global__ void __launch_bounds__(kApThreads) absolute_pose_ragged_kernel(AbsPos
     bool ok = false;
     if (i < len) {
       const size_t r = (size_t)r0 + i;
-      ok = (!a.mask || a.mask[r]) && finite3(a.x[2 * r]) && finite3(a.x[2 * r + 1]) && finite3(a.X[3 * r]) &&
-           finite3(a.X[3 * r + 1]) && finite3(a.X[3 * r + 2]);
+      ok = (!a.mask || a.mask[r]) && finite(a.x[2 * r]) && finite(a.x[2 * r + 1]) && finite(a.X[3 * r]) &&
+           finite(a.X[3 * r + 1]) && finite(a.X[3 * r + 2]);
       a.mask_out[r] = 0;
     }
     int total;
@@ -272,8 +262,8 @@ __global__ void __launch_bounds__(kApThreads) absolute_pose_ragged_kernel(AbsPos
     if (tid == 0) {
       a.n_inliers[p] = 0;
       a.iters[p] = s_iters;
-      a.cost0[p] = qnan3();
-      a.cost[p] = qnan3();
+      a.cost0[p] = qnan();
+      a.cost[p] = qnan();
     }
     return;
   }
@@ -341,7 +331,7 @@ __global__ void __launch_bounds__(kApThreads) absolute_pose_ragged_kernel(AbsPos
 
 extern "C" {
 
-const char* dgb200_absolute_pose_last_error(void) { return g_err3; }
+const char* dgb200_absolute_pose_last_error(void) { return g_err; }
 
 int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, const double* d_K, int k_per_pair,
                                          const int32_t* d_offsets, int n_pairs, int rows, const uint8_t* d_mask,
@@ -351,16 +341,16 @@ int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, c
                                          double* d_cost0_out, double* d_cost_out, void* stream) {
   if (!d_K || !d_offsets || !d_seeds || !d_R_out || !d_t_out || !d_n_inliers_out || !d_iters_out || !d_cost0_out ||
       !d_cost_out)
-    return fail3(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x || !d_X || !d_mask_out)) return fail3(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0) return fail3(DGB200_E_ARG, "need n_pairs >= 1 and rows >= 0");
-  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail3(DGB200_E_ARG, "px_th must be a positive number");
-  if (!(conf > 0.0 && conf <= 1.0)) return fail3(DGB200_E_ARG, "conf must lie in (0, 1]");
-  if (max_iters < 1) return fail3(DGB200_E_ARG, "max_iters must be at least 1");
-  if (refine_iters < 0) return fail3(DGB200_E_ARG, "refine_iters must not be negative");
+    return fail(DGB200_E_ARG, "null buffer");
+  if (rows > 0 && (!d_x || !d_X || !d_mask_out)) return fail(DGB200_E_ARG, "null row buffer");
+  if (n_pairs < 1 || rows < 0) return fail(DGB200_E_ARG, "need n_pairs >= 1 and rows >= 0");
+  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail(DGB200_E_ARG, "px_th must be a positive number");
+  if (!(conf > 0.0 && conf <= 1.0)) return fail(DGB200_E_ARG, "conf must lie in (0, 1]");
+  if (max_iters < 1) return fail(DGB200_E_ARG, "max_iters must be at least 1");
+  if (refine_iters < 0) return fail(DGB200_E_ARG, "refine_iters must not be negative");
   const cudaStream_t st = (cudaStream_t)stream;
   int* list = nullptr;
-  CU3(cudaMallocAsync((void**)&list, sizeof(int) * (size_t)(rows > 0 ? rows : 1), st));
+  CU(cudaMallocAsync((void**)&list, sizeof(int) * (size_t)(rows > 0 ? rows : 1), st));
   AbsPoseArgs a;
   a.x = d_x; a.X = d_X; a.K = d_K; a.k_per_pair = k_per_pair; a.offsets = d_offsets; a.mask = d_mask;
   a.n_pairs = n_pairs; a.rows = rows; a.max_iters = max_iters; a.refine_iters = refine_iters;
@@ -369,8 +359,8 @@ int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, c
   a.cost0 = d_cost0_out; a.cost = d_cost_out;
   absolute_pose_ragged_kernel<<<n_pairs, kApThreads, 0, st>>>(a);
   const cudaError_t launch = cudaGetLastError();
-  CU3(cudaFreeAsync(list, st));
-  CU3(launch);
+  CU(cudaFreeAsync(list, st));
+  CU(launch);
   return 0;
 }
 

@@ -28,39 +28,23 @@
 #include <stdio.h>
 
 #include "../../include/degensac_b200.h"
+#include "entry_error.h"
 #include "common.h"
 #include "absolute_pose.h"
 #include "pose_refine.h"
 #include "triangulate.h"
 #include "bundle_adjust.h"
+#include "device_util.h"
 
 namespace {
 
-thread_local char g_err5[256] = "";
-int fail5(int code, const char* what, cudaError_t e = cudaSuccess) {
-  if (e != cudaSuccess) snprintf(g_err5, sizeof(g_err5), "%s: %s", what, cudaGetErrorString(e));
-  else snprintf(g_err5, sizeof(g_err5), "%s", what);
-  return code;
-}
-#define CU5(call)                                                     \
-  do {                                                                \
-    cudaError_t e__ = (call);                                         \
-    if (e__ != cudaSuccess) return fail5(DGB200_E_CUDA, #call, e__);  \
-  } while (0)
+thread_local char g_err[256] = "";
+int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_error(g_err, code, what, e); }
 
 constexpr int kBaWarps = 4;                       // tracks (or Schur blocks) per CTA, one per warp
 constexpr int kBaThreads = 32 * kBaWarps;
 constexpr int kBaCamThreads = 128;
 constexpr int kBaCta = 1024;                      // the one-CTA kernels and the per-slot scans
-constexpr unsigned kFull = 0xffffffffu;
-
-__device__ __forceinline__ bool finite5(double v) { return fabs(v) < INFINITY; }
-
-template <typename T>
-__device__ __forceinline__ T warp_sum5(T v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
-}
 
 // The LM state of the call, in the workspace; only ba_init_kernel and ba_decide_kernel write it (bad: also the
 // kernels that find a non-positive pivot)
@@ -140,7 +124,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_mark_kernel(BaArgs a) {
   }
   const int b = a.offsets[j], e = a.offsets[j + 1];
   if (!span_ok(a, b, e)) return;                     // malformed span: no row read or written
-  const bool xok = finite5(X[0]) && finite5(X[1]) && finite5(X[2]);
+  const bool xok = finite(X[0]) && finite(X[1]) && finite(X[2]);
   // the usable observations; the camera of the first one and whether another camera sees the track too
   int first_cam = -1, n = 0;
   bool two = false;
@@ -152,7 +136,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_mark_kernel(BaArgs a) {
     if (r < e) {
       cm = a.cams[r];
       const double x = a.pts[2 * (size_t)r], y = a.pts[2 * (size_t)r + 1];
-      ok = xok && (!a.mask || a.mask[r]) && cm >= 0 && cm < a.n_cams && finite5(x) && finite5(y) &&
+      ok = xok && (!a.mask || a.mask[r]) && cm >= 0 && cm < a.n_cams && finite(x) && finite(y) &&
            a.tab[dg::kTrCamStride * (size_t)cm + dg::kTrCamOk] != 0.0;
       if (ok) {
         const double* P = pose_of(a, 0, cm);
@@ -178,8 +162,8 @@ __global__ void __launch_bounds__(kBaThreads) ba_mark_kernel(BaArgs a) {
     n += __popc(bal);
   }
 #pragma unroll
-  for (int s = 0; s < 6; ++s) V[s] = warp_sum5(V[s]);
-  cost = warp_sum5(cost);
+  for (int s = 0; s < 6; ++s) V[s] = warp_sum(V[s]);
+  cost = warp_sum(cost);
   double Vi[6];
   const bool opt = two && dg::ba_inv3(V, 0.0, Vi);
   __syncwarp();
@@ -196,7 +180,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_mark_kernel(BaArgs a) {
 
 __device__ int block_sum_int(int v, int* sh) {
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  v = warp_sum5(v);
+  v = warp_sum(v);
   if (lane == 0) sh[wid] = v;
   __syncthreads();
   int total = 0;
@@ -312,9 +296,9 @@ __global__ void __launch_bounds__(kBaThreads) ba_linearise_kernel(BaArgs a) {
     if (a.slot_of[cm] >= 0) dg::ba_cross_block(o + dg::kBaObsJc, Jx, w, o + dg::kBaObsWm);
   }
 #pragma unroll
-  for (int s = 0; s < 6; ++s) V[s] = warp_sum5(V[s]);
+  for (int s = 0; s < 6; ++s) V[s] = warp_sum(V[s]);
 #pragma unroll
-  for (int s = 0; s < 3; ++s) g[s] = warp_sum5(g[s]);
+  for (int s = 0; s < 3; ++s) g[s] = warp_sum(g[s]);
   if (lane == 0) {
     double* tk = a.trk + dg::kBaTrkStride * (size_t)j;
 #pragma unroll
@@ -396,9 +380,9 @@ __global__ void __launch_bounds__(kBaThreads) ba_schur_kernel(BaArgs a) {
         h[k] += w * (Jc[k] * e0 + Jc[6 + k] * e1) - (Y[3 * k] * gp[0] + Y[3 * k + 1] * gp[1] + Y[3 * k + 2] * gp[2]);
     }
 #pragma unroll
-    for (int s = 0; s < 21; ++s) U[s] = warp_sum5(U[s]);
+    for (int s = 0; s < 21; ++s) U[s] = warp_sum(U[s]);
 #pragma unroll
-    for (int s = 0; s < 6; ++s) h[s] = warp_sum5(h[s]);
+    for (int s = 0; s < 6; ++s) h[s] = warp_sum(h[s]);
     if (lane == 0) {
       const double lam = st->lam;
       int m = 0;
@@ -435,7 +419,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_schur_kernel(BaArgs a) {
     }
   }
 #pragma unroll
-  for (int s = 0; s < 36; ++s) M[s] = warp_sum5(M[s]);
+  for (int s = 0; s < 36; ++s) M[s] = warp_sum(M[s]);
   __syncwarp();                                        // lane 0's U*_a is written
   if (lane == 0) {
 #pragma unroll
@@ -532,7 +516,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_backsub_kernel(BaArgs a) {
       for (int k = 0; k < 6; ++k) acc[m] += W[3 * k + m] * d[k];
   }
 #pragma unroll
-  for (int m = 0; m < 3; ++m) acc[m] = warp_sum5(acc[m]);
+  for (int m = 0; m < 3; ++m) acc[m] = warp_sum(acc[m]);
   const double* tk = a.trk + dg::kBaTrkStride * (size_t)j;
   const double v[3] = {tk[dg::kBaTrkG] + acc[0], tk[dg::kBaTrkG + 1] + acc[1], tk[dg::kBaTrkG + 2] + acc[2]};
   double D[3];
@@ -549,7 +533,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_backsub_kernel(BaArgs a) {
                                       a.pts[2 * (size_t)r], a.pts[2 * (size_t)r + 1], X[0], X[1], X[2], &front);
     c += front ? dg::ba_rho(e2, a.sig2) : INFINITY;
   }
-  c = warp_sum5(c);
+  c = warp_sum(c);
   if (lane == 0) a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost] = c;
 }
 
@@ -632,7 +616,7 @@ T* carve(char*& p, size_t count) {
 
 extern "C" {
 
-const char* dgb200_bundle_adjust_last_error(void) { return g_err5; }
+const char* dgb200_bundle_adjust_last_error(void) { return g_err; }
 
 int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R, const double* d_t,
                                     const double* d_K, int k_per_camera, int n_cams, const int32_t* d_offsets,
@@ -643,31 +627,31 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
                                     int32_t* d_iters_out, int32_t* d_n_used_out, void* stream) {
   if (!d_R || !d_t || !d_K || !d_offsets || !d_X || !d_R_out || !d_t_out || !d_X_out || !d_cost0_out ||
       !d_cost_out || !d_iters_out || !d_n_used_out)
-    return fail5(DGB200_E_ARG, "null buffer");
-  if (obs > 0 && (!d_cams || !d_pts || !d_mask_out)) return fail5(DGB200_E_ARG, "null observation buffer");
-  if (n_tracks < 1 || obs < 0 || n_cams < 1) return fail5(DGB200_E_ARG, "need n_tracks >= 1, obs >= 0 and n_cams >= 1");
-  if (n_free < 0 || n_free > dg::kBaMaxFree) return fail5(DGB200_E_ARG, "n_free must lie in [0, 64]");
-  if (n_free > 0 && !h_free) return fail5(DGB200_E_ARG, "null free-camera list");
+    return fail(DGB200_E_ARG, "null buffer");
+  if (obs > 0 && (!d_cams || !d_pts || !d_mask_out)) return fail(DGB200_E_ARG, "null observation buffer");
+  if (n_tracks < 1 || obs < 0 || n_cams < 1) return fail(DGB200_E_ARG, "need n_tracks >= 1, obs >= 0 and n_cams >= 1");
+  if (n_free < 0 || n_free > dg::kBaMaxFree) return fail(DGB200_E_ARG, "n_free must lie in [0, 64]");
+  if (n_free > 0 && !h_free) return fail(DGB200_E_ARG, "null free-camera list");
   int gauge_slot = -1;
   for (int q = 0; q < n_free; ++q) {
-    if (h_free[q] < 0 || h_free[q] >= n_cams) return fail5(DGB200_E_ARG, "free camera index out of range");
+    if (h_free[q] < 0 || h_free[q] >= n_cams) return fail(DGB200_E_ARG, "free camera index out of range");
     for (int p = 0; p < q; ++p)
-      if (h_free[p] == h_free[q]) return fail5(DGB200_E_ARG, "free camera index repeated");
+      if (h_free[p] == h_free[q]) return fail(DGB200_E_ARG, "free camera index repeated");
     if (h_free[q] == scale_gauge) gauge_slot = q;
   }
-  if (scale_gauge >= 0 && gauge_slot < 0) return fail5(DGB200_E_ARG, "scale_gauge must be one of the free cameras");
-  if (scale_gauge < -1) return fail5(DGB200_E_ARG, "scale_gauge must be a free camera or -1");
+  if (scale_gauge >= 0 && gauge_slot < 0) return fail(DGB200_E_ARG, "scale_gauge must be one of the free cameras");
+  if (scale_gauge < -1) return fail(DGB200_E_ARG, "scale_gauge must be a free camera or -1");
   int held_cam = -1;                                   // the lowest-index camera outside the free list
   for (int c = 0; c < n_cams && held_cam < 0; ++c) {
     bool is_free = false;
     for (int q = 0; q < n_free; ++q) is_free = is_free || h_free[q] == c;
     if (!is_free) held_cam = c;
   }
-  if (gauge_slot >= 0 && held_cam < 0) return fail5(DGB200_E_ARG, "scale_gauge needs a held camera");
+  if (gauge_slot >= 0 && held_cam < 0) return fail(DGB200_E_ARG, "scale_gauge needs a held camera");
   if (!(loss_scale >= 0.0) || !(loss_scale < INFINITY))
-    return fail5(DGB200_E_ARG, "loss_scale must be a positive number (or 0 for the trivial loss)");
-  if (max_iters < 0) return fail5(DGB200_E_ARG, "max_iters must not be negative");
-  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail5(DGB200_E_ARG, "px_th must be a positive number");
+    return fail(DGB200_E_ARG, "loss_scale must be a positive number (or 0 for the trivial loss)");
+  if (max_iters < 0) return fail(DGB200_E_ARG, "max_iters must not be negative");
+  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail(DGB200_E_ARG, "px_th must be a positive number");
   const cudaStream_t st = (cudaStream_t)stream;
   const int n = dg::kBaCamParams * n_free;
   const size_t no = (size_t)(obs > 0 ? obs : 1), nt = (size_t)n_tracks, nc = (size_t)n_cams;
@@ -676,7 +660,7 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
                                                     dg::kBaTrkStride * nt + nn * nn + nn) +
                        sizeof(BaState) + sizeof(int) * (nc + 2 * no + 2 * (size_t)n_free + 1 + nt) + 2 * no;
   char* ws = nullptr;
-  CU5(cudaMallocAsync((void**)&ws, bytes, st));
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
   BaArgs a;
   a.cams = d_cams; a.pts = d_pts; a.R = d_R; a.t = d_t; a.K = d_K; a.k_per_camera = k_per_camera; a.n_cams = n_cams;
   a.offsets = d_offsets; a.mask = d_mask; a.X = d_X; a.n_tracks = n_tracks; a.obs = obs; a.n_free = n_free; a.n = n;
@@ -735,8 +719,8 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
   L5((ba_finish_cameras_kernel<<<cam_grid, kBaCamThreads, 0, st>>>(a)));
   L5((ba_finish_tracks_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
 #undef L5
-  CU5(cudaFreeAsync(ws, st));
-  CU5(launch);
+  CU(cudaFreeAsync(ws, st));
+  CU(launch);
   return 0;
 }
 

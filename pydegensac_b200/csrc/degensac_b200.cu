@@ -22,6 +22,7 @@
 #include <string.h>
 
 #include "../../include/degensac_b200.h"
+#include "entry_error.h"
 #include "engine_f.h"
 #include "engine_h.h"
 #include "engine_h2el.h"
@@ -274,16 +275,7 @@ thread_local char g_err[512] = "";
 long long g_launches = 0;
 double g_last_ms = 0.0;
 
-int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
-  if (e != cudaSuccess) snprintf(g_err, sizeof(g_err), "%s: %s", what, cudaGetErrorString(e));
-  else snprintf(g_err, sizeof(g_err), "%s", what);
-  return code;
-}
-#define CU(call)                                                     \
-  do {                                                               \
-    cudaError_t e__ = (call);                                        \
-    if (e__ != cudaSuccess) return fail(DGB200_E_CUDA, #call, e__);  \
-  } while (0)
+int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_error(g_err, code, what, e); }
 
 void destroy_device_state() {   // with the owning device current
   for (LaunchCtx& x : g_c.ctxs) {

@@ -24,6 +24,7 @@
 #include <vector>
 
 #include "../../include/degensac_b200.h"
+#include "entry_error.h"
 #include "common.h"
 #include "la.h"
 #include "hgeom.h"
@@ -31,20 +32,12 @@
 #include "refine_h.h"
 #include "refine_f.h"
 #include "rng.h"
+#include "device_util.h"
 
 namespace {
 
-thread_local char g_err2[256] = "";
-int fail2(int code, const char* what, cudaError_t e = cudaSuccess) {
-  if (e != cudaSuccess) snprintf(g_err2, sizeof(g_err2), "%s: %s", what, cudaGetErrorString(e));
-  else snprintf(g_err2, sizeof(g_err2), "%s", what);
-  return code;
-}
-#define CU2(call)                                                     \
-  do {                                                                \
-    cudaError_t e__ = (call);                                         \
-    if (e__ != cudaSuccess) return fail2(DGB200_E_CUDA, #call, e__);  \
-  } while (0)
+thread_local char g_err[256] = "";
+int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_error(g_err, code, what, e); }
 
 // ------------------------------------------------------------------------------------------------ matcher
 constexpr int kTQ = 32;          // query descriptors per CTA
@@ -112,8 +105,6 @@ struct NoGate {             // plain matching: every train descriptor is a candi
   static constexpr int kTerms = 0;
   struct Q {};
 };
-
-__device__ __forceinline__ double qnan() { return __longlong_as_double(0x7ff8000000000000ll); }
 
 // F (x_t^T F x_q = 0): the engine's Sampson residual dg::f_resid_sampson(F, xq, yq, xt, yt) <= th -- the rule that
 // makes a correspondence an inlier of the RANSAC mask.  f_res_terms: rxc, ryc, rwc depend on the train point only, rx,
@@ -1579,18 +1570,18 @@ size_t match_ws_bytes(long long sum_n1, long long sum_n2, int n_pairs) {
 // table [n_pairs][2] = (query image, train image).  Rejects malformed input; meta[n_pairs] holds the totals.
 int build_meta(const int32_t* qoff, const int32_t* toff, int n_images, const int32_t* pairs, int n_pairs,
                std::vector<PairMeta>* meta) {
-  if (!qoff || !toff || !pairs) return fail2(DGB200_E_ARG, "null image offsets or pair table");
-  if (n_images < 1 || n_pairs < 1) return fail2(DGB200_E_ARG, "need n_images >= 1 and n_pairs >= 1");
+  if (!qoff || !toff || !pairs) return fail(DGB200_E_ARG, "null image offsets or pair table");
+  if (n_images < 1 || n_pairs < 1) return fail(DGB200_E_ARG, "need n_images >= 1 and n_pairs >= 1");
   for (const int32_t* off : {qoff, toff}) {
-    if (off[0] != 0) return fail2(DGB200_E_ARG, "image offsets must start at 0");
+    if (off[0] != 0) return fail(DGB200_E_ARG, "image offsets must start at 0");
     for (int i = 0; i < n_images; ++i)
-      if (off[i + 1] < off[i]) return fail2(DGB200_E_ARG, "image offsets must be non-decreasing");
+      if (off[i + 1] < off[i]) return fail(DGB200_E_ARG, "image offsets must be non-decreasing");
   }
   meta->assign((size_t)n_pairs + 1, PairMeta{});
   long long tiles = 0, rows = 0, cols = 0;
   for (int p = 0; p < n_pairs; ++p) {
     const int qi = pairs[2 * p], ti = pairs[2 * p + 1];
-    if (qi < 0 || qi >= n_images || ti < 0 || ti >= n_images) return fail2(DGB200_E_ARG, "pair table: image index out of range");
+    if (qi < 0 || qi >= n_images || ti < 0 || ti >= n_images) return fail(DGB200_E_ARG, "pair table: image index out of range");
     PairMeta& m = (*meta)[p];
     m.qrow = qoff[qi]; m.n1 = qoff[qi + 1] - qoff[qi];
     m.trow = toff[ti]; m.n2 = toff[ti + 1] - toff[ti];
@@ -1598,7 +1589,7 @@ int build_meta(const int32_t* qoff, const int32_t* toff, int n_images, const int
     if (m.n1 >= 1 && m.n2 >= 2) tiles += (m.n1 + kTQ - 1) / kTQ;   // degenerate pairs: no work, zero matches
     rows += m.n1;
     cols += m.n2;
-    if (rows > INT32_MAX || cols > INT32_MAX) return fail2(DGB200_E_ARG, "batch too large: more than 2^31 - 1 rows");
+    if (rows > INT32_MAX || cols > INT32_MAX) return fail(DGB200_E_ARG, "batch too large: more than 2^31 - 1 rows");
   }
   PairMeta& e = (*meta)[n_pairs];
   e.tile0 = (int)tiles; e.row0 = (int)rows; e.col0 = (int)cols;
@@ -1633,9 +1624,9 @@ int run_match(const void* qbank, const void* tbank, int D, int hamming, const st
   a.mutual = mutual;
   a.models = models; a.kq = kq; a.kt = kt; a.kp_dim = kp_dim; a.th = th;
   // pageable source: the runtime stages it before returning, the copy itself is ordered on st like the kernels
-  CU2(cudaMemcpyAsync(d_meta, meta.data(), sizeof(PairMeta) * meta.size(), cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(d_meta, meta.data(), sizeof(PairMeta) * meta.size(), cudaMemcpyHostToDevice, st));
   if (tot.tile0 > 0) {
-    if (mutual) CU2(cudaMemsetAsync(a.col_best, 0xff, sizeof(unsigned long long) * (size_t)tot.col0, st));
+    if (mutual) CU(cudaMemsetAsync(a.col_best, 0xff, sizeof(unsigned long long) * (size_t)tot.col0, st));
     void (*kern)(MatchArgs);
     size_t smem;
     if (guide == DGB200_GUIDE_F) {
@@ -1648,23 +1639,23 @@ int run_match(const void* qbank, const void* tbank, int D, int hamming, const st
       kern = hamming ? nn2_kernel<HammingDist, NoGate> : nn2_kernel<L2Dist, NoGate>;
       smem = nn2_smem_bytes(D, 0);
     }
-    CU2(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kern<<<tot.tile0, kMatchThreads, smem, st>>>(a);
-    CU2(cudaGetLastError());
+    CU(cudaGetLastError());
   }
   SelectArgs s;
   s.meta = d_meta; s.nn_idx = a.nn_idx; s.nn_d1 = a.nn_d1; s.nn_d2 = a.nn_d2; s.col_best = a.col_best;
   s.ratio2 = (float)ratio * (float)ratio; s.mutual = mutual; s.counts = counts;
   s.hamming = hamming; s.ratio = ratio;
   count_kernel<<<P, kSelThreads, 0, st>>>(s);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   scan_kernel<<<1, 1024, 0, st>>>(counts, P, offsets, cap, count_out);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   WriteArgs wa;
   wa.s = s; wa.offsets = offsets; wa.kq = kq; wa.kt = kt; wa.kp_dim = kp_dim;
   wa.match_q = match_q; wa.match_t = match_t; wa.x1y1 = x1y1; wa.x2y2 = x2y2; wa.out_dim = out_dim; wa.cap = cap;
   write_kernel<<<P, kSelThreads, 0, st>>>(wa);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -1683,10 +1674,10 @@ int match_single(const void* d_desc1, int n1, const void* d_desc2, int n2, int D
                  double ratio, int mutual, const double* d_kp1, const double* d_kp2, int kp_dim, int* d_match_q,
                  int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim, int capacity, int* d_count,
                  void* d_workspace, void* stream) {
-  if (!d_desc1 || !d_desc2 || !d_match_q || !d_match_t || !d_count || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
-  if (n1 < 1 || n2 < 2) return fail2(DGB200_E_ARG, "need n1 >= 1 query and n2 >= 2 train descriptors");
-  if (len_err) return fail2(DGB200_E_ARG, len_err);
-  if (d_x1y1 && (!d_kp1 || !d_kp2 || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  if (!d_desc1 || !d_desc2 || !d_match_q || !d_match_t || !d_count || !d_workspace) return fail(DGB200_E_ARG, "null buffer");
+  if (n1 < 1 || n2 < 2) return fail(DGB200_E_ARG, "need n1 >= 1 query and n2 >= 2 train descriptors");
+  if (len_err) return fail(DGB200_E_ARG, len_err);
+  if (d_x1y1 && (!d_kp1 || !d_kp2 || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
   const int32_t qoff[3] = {0, n1, n1}, toff[3] = {0, 0, n2}, pair[2] = {0, 1};
   std::vector<PairMeta> meta;
   const int rc = build_meta(qoff, toff, 2, pair, 1, &meta);
@@ -1701,20 +1692,20 @@ int match_batch(const void* d_bank, const int32_t* img_offsets, int n_images, in
                 int* d_match_q, int* d_match_t, double* d_x1y1, double* d_x2y2, int out_dim, int capacity,
                 int32_t* d_offsets_out, void* d_workspace, void* stream, bool guided = false, int guide = kNoGuide,
                 const double* d_models = nullptr, double px_th = 0.0) {
-  if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail2(DGB200_E_ARG, "null buffer");
-  if (len_err) return fail2(DGB200_E_ARG, len_err);
-  if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail2(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
+  if (!d_match_q || !d_match_t || !d_offsets_out || !d_workspace) return fail(DGB200_E_ARG, "null buffer");
+  if (len_err) return fail(DGB200_E_ARG, len_err);
+  if (d_x1y1 && (!d_kp_bank || !d_x2y2 || out_dim < 2 || out_dim > kp_dim)) return fail(DGB200_E_ARG, "keypoint arrays / out_dim inconsistent");
   if (guided) {
-    if (!d_models) return fail2(DGB200_E_ARG, "null model array");
-    if (!d_kp_bank || kp_dim < 2) return fail2(DGB200_E_ARG, "guided matching needs the keypoint bank (kp_dim >= 2)");
-    if (guide != DGB200_GUIDE_F && guide != DGB200_GUIDE_H) return fail2(DGB200_E_ARG, "guide must be DGB200_GUIDE_F or DGB200_GUIDE_H");
-    if (!(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+    if (!d_models) return fail(DGB200_E_ARG, "null model array");
+    if (!d_kp_bank || kp_dim < 2) return fail(DGB200_E_ARG, "guided matching needs the keypoint bank (kp_dim >= 2)");
+    if (guide != DGB200_GUIDE_F && guide != DGB200_GUIDE_H) return fail(DGB200_E_ARG, "guide must be DGB200_GUIDE_F or DGB200_GUIDE_H");
+    if (!(px_th >= 0.0)) return fail(DGB200_E_ARG, "px_th must be a non-negative number");
   }
   std::vector<PairMeta> meta;
   const int rc = build_meta(img_offsets, img_offsets, n_images, pairs, n_pairs, &meta);
   if (rc) return rc;
-  if (!d_bank && meta[n_pairs].tile0 > 0) return fail2(DGB200_E_ARG, "null descriptor bank");
-  if (capacity < meta[n_pairs].row0) return fail2(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
+  if (!d_bank && meta[n_pairs].tile0 > 0) return fail(DGB200_E_ARG, "null descriptor bank");
+  if (capacity < meta[n_pairs].row0) return fail(DGB200_E_ARG, "capacity below the sum of the query images' descriptor counts");
   return run_match(d_bank, d_bank, D, hamming, meta, ratio, mutual, d_kp_bank, d_kp_bank, kp_dim, d_match_q, d_match_t,
                    d_x1y1, d_x2y2, out_dim, capacity, d_offsets_out, nullptr, d_workspace, (cudaStream_t)stream,
                    guided ? guide : kNoGuide, d_models, px_th * px_th);
@@ -1730,22 +1721,51 @@ PoseRows pose_rows_args(const double* K1, const double* K2, int k_per_pair, cons
   return w;
 }
 
+// The checks the ragged pose and refine entry points share, in their order, after each has refused its null required
+// buffers: the message of the first that fails, or nullptr.  row_bufs: every row buffer is non-null (needed only when
+// rows > 0).  The pose calls pass max_iters = 0 and no inliers.
+const char* ragged_arg_error(int n_pairs, int rows, int dim, bool row_bufs, int max_iters, bool inliers, double px_th) {
+  if (rows > 0 && !row_bufs) return "null row buffer";
+  if (n_pairs < 1 || rows < 0 || dim < 2) return "need n_pairs >= 1, rows >= 0 and dim >= 2";
+  if (max_iters < 0) return "max_iters must not be negative";
+  if (inliers && !(px_th >= 0.0)) return "px_th must be a non-negative number";
+  return nullptr;
+}
+
+// The refinement of one 3 x 3 model per pair (H or F) by `kernel`
+int refine_model_ragged(void (*kernel)(RefineArgs), const double* d_M, const double* d_x1y1, const double* d_x2y2,
+                        const int32_t* d_offsets, int n_pairs, int rows, int dim, const uint8_t* d_mask, int max_iters,
+                        double px_th, double* d_M_out, double* d_cost0_out, double* d_cost_out, int32_t* d_n_used_out,
+                        int32_t* d_iters_out, uint8_t* d_inliers_out, void* stream) {
+  if (!d_M || !d_offsets || !d_M_out || !d_cost_out) return fail(DGB200_E_ARG, "null buffer");
+  if (const char* err = ragged_arg_error(n_pairs, rows, dim, d_x1y1 && d_x2y2, max_iters, d_inliers_out, px_th))
+    return fail(DGB200_E_ARG, err);
+  RefineArgs a;
+  a.model = d_M; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
+  a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
+  a.model_out = d_M_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
+  a.inliers = d_inliers_out;
+  kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
+  CU(cudaGetLastError());
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
 
 int dgb200_debug_div_check(unsigned long long seed, long long count, unsigned long long* h_bad) {
   unsigned long long* d = nullptr;
-  CU2(cudaMalloc(&d, sizeof(unsigned long long)));
-  CU2(cudaMemset(d, 0, sizeof(unsigned long long)));
+  CU(cudaMalloc(&d, sizeof(unsigned long long)));
+  CU(cudaMemset(d, 0, sizeof(unsigned long long)));
   div_check_kernel<<<1184, 256>>>(seed, count, d);
-  CU2(cudaGetLastError());
-  CU2(cudaMemcpy(h_bad, d, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+  CU(cudaGetLastError());
+  CU(cudaMemcpy(h_bad, d, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   cudaFree(d);
   return 0;
 }
 
-const char* dgb200_frontend_last_error(void) { return g_err2; }
+const char* dgb200_frontend_last_error(void) { return g_err; }
 
 size_t dgb200_match_workspace_bytes(int n1, int n2) {
   if (n1 < 0 || n2 < 0) return 0;
@@ -1820,14 +1840,14 @@ int dgb200_pose_from_fundamental_batch_dev(const double* d_F,const double* d_K1,
                                            const double* d_x1y1, const double* d_x2y2, const uint8_t* d_mask, int n_pairs,
                                            int n, int dim, double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                            void* stream) {
-  if (!d_F || !d_K1 || !d_K2 || !d_x1y1 || !d_x2y2 || !d_R_out || !d_t_out) return fail2(DGB200_E_ARG, "null buffer");
-  if (n_pairs < 1 || n < 1 || dim < 2) return fail2(DGB200_E_ARG, "bad sizes");
+  if (!d_F || !d_K1 || !d_K2 || !d_x1y1 || !d_x2y2 || !d_R_out || !d_t_out) return fail(DGB200_E_ARG, "null buffer");
+  if (n_pairs < 1 || n < 1 || dim < 2) return fail(DGB200_E_ARG, "bad sizes");
   PoseArgs a;
   a.F = d_F; a.K1 = d_K1; a.K2 = d_K2; a.k_per_pair = k_per_pair; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.mask = d_mask;
   a.n_pairs = n_pairs; a.n = n; a.dim = dim; a.R = d_R_out; a.t = d_t_out; a.good = d_good_out;
   const int threads = 256;
   pose_kernel<<<(n_pairs * 32 + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -1837,16 +1857,16 @@ int dgb200_pose_from_fundamental_ragged_dev(const double* d_F, const double* d_K
                                             double* d_R_out, double* d_t_out, int32_t* d_good_out,
                                             double* d_points_out, uint8_t* d_in_front_out, double* d_angle_out,
                                             double* d_median_angle_out, void* stream) {
-  if (!d_F || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_median_angle_out) return fail2(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x1y1 || !d_x2y2 || !d_points_out || !d_in_front_out || !d_angle_out))
-    return fail2(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+  if (!d_F || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_median_angle_out) return fail(DGB200_E_ARG, "null buffer");
+  if (const char* err = ragged_arg_error(n_pairs, rows, dim,
+                                         d_x1y1 && d_x2y2 && d_points_out && d_in_front_out && d_angle_out, 0, false, 0.0))
+    return fail(DGB200_E_ARG, err);
   PoseRaggedArgs a;
   a.w = pose_rows_args(d_K1, d_K2, k_per_pair, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask, d_points_out,
                        d_in_front_out, d_angle_out, d_median_angle_out);
   a.F = d_F; a.R = d_R_out; a.t = d_t_out; a.good = d_good_out;
   pose_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -1858,17 +1878,17 @@ int dgb200_pose_from_homography_ragged_dev(const double* d_H, const double* d_K1
                                            double* d_angle_out, double* d_median_angle_out, void* stream) {
   if (!d_H || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_plane_out || !d_rotation_only_out ||
       !d_median_angle_out)
-    return fail2(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x1y1 || !d_x2y2 || !d_points_out || !d_in_front_out || !d_angle_out))
-    return fail2(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
+    return fail(DGB200_E_ARG, "null buffer");
+  if (const char* err = ragged_arg_error(n_pairs, rows, dim,
+                                         d_x1y1 && d_x2y2 && d_points_out && d_in_front_out && d_angle_out, 0, false, 0.0))
+    return fail(DGB200_E_ARG, err);
   PoseHRaggedArgs a;
   a.w = pose_rows_args(d_K1, d_K2, k_per_pair, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask, d_points_out,
                        d_in_front_out, d_angle_out, d_median_angle_out);
   a.H = d_H; a.R = d_R_out; a.t = d_t_out; a.plane = d_plane_out; a.good = d_good_out;
   a.rotation_only = d_rotation_only_out;
   pose_h_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -1879,11 +1899,9 @@ int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const do
                                   double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                   uint8_t* d_inliers_out, void* stream) {
   if (!d_R || !d_t || !d_K1 || !d_K2 || !d_offsets || !d_R_out || !d_t_out || !d_F_out || !d_cost_out)
-    return fail2(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
-  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
-  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
+    return fail(DGB200_E_ARG, "null buffer");
+  if (const char* err = ragged_arg_error(n_pairs, rows, dim, d_x1y1 && d_x2y2, max_iters, d_inliers_out, px_th))
+    return fail(DGB200_E_ARG, err);
   PoseRefineArgs a;
   a.R = d_R; a.t = d_t; a.K1 = d_K1; a.K2 = d_K2; a.k_per_pair = k_per_pair; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2;
   a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs; a.rows = rows; a.dim = dim; a.max_iters = max_iters;
@@ -1891,7 +1909,7 @@ int dgb200_refine_pose_ragged_dev(const double* d_R, const double* d_t, const do
   a.R_out = d_R_out; a.t_out = d_t_out; a.F_out = d_F_out; a.cost0 = d_cost0_out; a.cost = d_cost_out;
   a.n_used = d_n_used_out; a.iters = d_iters_out; a.inliers = d_inliers_out;
   pose_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 
@@ -1900,19 +1918,9 @@ int dgb200_refine_homography_ragged_dev(const double* d_H, const double* d_x1y1,
                                         int max_iters, double px_th, double* d_H_out, double* d_cost0_out,
                                         double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                         uint8_t* d_inliers_out, void* stream) {
-  if (!d_H || !d_offsets || !d_H_out || !d_cost_out) return fail2(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
-  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
-  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
-  RefineArgs a;
-  a.model = d_H; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
-  a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
-  a.model_out = d_H_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
-  a.inliers = d_inliers_out;
-  h_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
-  return 0;
+  return refine_model_ragged(h_refine_ragged_kernel, d_H, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask,
+                             max_iters, px_th, d_H_out, d_cost0_out, d_cost_out, d_n_used_out, d_iters_out,
+                             d_inliers_out, stream);
 }
 
 int dgb200_refine_fundamental_ragged_dev(const double* d_F, const double* d_x1y1, const double* d_x2y2,
@@ -1920,25 +1928,15 @@ int dgb200_refine_fundamental_ragged_dev(const double* d_F, const double* d_x1y1
                                          int max_iters, double px_th, double* d_F_out, double* d_cost0_out,
                                          double* d_cost_out, int32_t* d_n_used_out, int32_t* d_iters_out,
                                          uint8_t* d_inliers_out, void* stream) {
-  if (!d_F || !d_offsets || !d_F_out || !d_cost_out) return fail2(DGB200_E_ARG, "null buffer");
-  if (rows > 0 && (!d_x1y1 || !d_x2y2)) return fail2(DGB200_E_ARG, "null row buffer");
-  if (n_pairs < 1 || rows < 0 || dim < 2) return fail2(DGB200_E_ARG, "need n_pairs >= 1, rows >= 0 and dim >= 2");
-  if (max_iters < 0) return fail2(DGB200_E_ARG, "max_iters must not be negative");
-  if (d_inliers_out && !(px_th >= 0.0)) return fail2(DGB200_E_ARG, "px_th must be a non-negative number");
-  RefineArgs a;
-  a.model = d_F; a.x1y1 = d_x1y1; a.x2y2 = d_x2y2; a.offsets = d_offsets; a.mask = d_mask; a.n_pairs = n_pairs;
-  a.rows = rows; a.dim = dim; a.max_iters = max_iters; a.th2 = d_inliers_out ? px_th * px_th : 0.0;
-  a.model_out = d_F_out; a.cost0 = d_cost0_out; a.cost = d_cost_out; a.n_used = d_n_used_out; a.iters = d_iters_out;
-  a.inliers = d_inliers_out;
-  f_refine_ragged_kernel<<<n_pairs, kPoseThreads, 0, (cudaStream_t)stream>>>(a);
-  CU2(cudaGetLastError());
-  return 0;
+  return refine_model_ragged(f_refine_ragged_kernel, d_F, d_x1y1, d_x2y2, d_offsets, n_pairs, rows, dim, d_mask,
+                             max_iters, px_th, d_F_out, d_cost0_out, d_cost_out, d_n_used_out, d_iters_out,
+                             d_inliers_out, stream);
 }
 
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream) {
-  if (!d_A || !d_N || count < 1) return fail2(DGB200_E_ARG, "bad arguments");
+  if (!d_A || !d_N || count < 1) return fail(DGB200_E_ARG, "bad arguments");
   qr7x9_kernel<<<(count + 127) / 128, 128, 0, (cudaStream_t)stream>>>(d_A, d_N, d_rc, count);
-  CU2(cudaGetLastError());
+  CU(cudaGetLastError());
   return 0;
 }
 

@@ -22,33 +22,22 @@
 #include <stdio.h>
 
 #include "../../include/degensac_b200.h"
+#include "entry_error.h"
 #include "common.h"
 #include "rng.h"
 #include "absolute_pose.h"
 #include "pose_refine.h"
 #include "triangulate.h"
+#include "device_util.h"
 
 namespace {
 
-thread_local char g_err4[256] = "";
-int fail4(int code, const char* what, cudaError_t e = cudaSuccess) {
-  if (e != cudaSuccess) snprintf(g_err4, sizeof(g_err4), "%s: %s", what, cudaGetErrorString(e));
-  else snprintf(g_err4, sizeof(g_err4), "%s", what);
-  return code;
-}
-#define CU4(call)                                                     \
-  do {                                                                \
-    cudaError_t e__ = (call);                                         \
-    if (e__ != cudaSuccess) return fail4(DGB200_E_CUDA, #call, e__);  \
-  } while (0)
+thread_local char g_err[256] = "";
+int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_error(g_err, code, what, e); }
 
 constexpr int kTrWarps = 4;                       // tracks per CTA, one per warp
 constexpr int kTrThreads = 32 * kTrWarps;
 constexpr int kTrCamThreads = 128;
-constexpr unsigned kFull = 0xffffffffu;
-
-__device__ __forceinline__ double qnan4() { return __longlong_as_double(0x7ff8000000000000ll); }
-__device__ __forceinline__ bool finite4(double v) { return fabs(v) < INFINITY; }
 
 struct TriArgs {
   const int* cams; const double* pts; const double* tab;   // [obs], [obs][2], camera table [n_cams][kTrCamStride]
@@ -69,12 +58,6 @@ __global__ void __launch_bounds__(kTrCamThreads) triangulate_cameras_kernel(cons
   if (c >= n_cams) return;
   dg::tr_camera(R + 9 * (size_t)c, t + 3 * (size_t)c, K + (k_per_camera ? 9 * (size_t)c : 0),
                 tab + dg::kTrCamStride * (size_t)c);
-}
-
-template <typename T>
-__device__ __forceinline__ T warp_sum(T v) {
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  return v;
 }
 
 struct Select { double cost; int inliers, changed; };
@@ -133,13 +116,13 @@ __global__ void __launch_bounds__(kTrThreads) triangulate_tracks_ragged_kernel(T
   if (j >= a.n_tracks) return;                       // (warp-uniform)
   const int b = a.offsets[j], e = a.offsets[j + 1];
   if (!(b >= 0 && b <= e && e <= a.obs)) {           // malformed span: no model, no row read or written
-    if (lane < 3) a.X_out[3 * (size_t)j + lane] = qnan4();
+    if (lane < 3) a.X_out[3 * (size_t)j + lane] = qnan();
     if (lane == 0) {
       a.n_inliers[j] = 0;
       a.iters[j] = 0;
-      a.cost0[j] = qnan4();
-      a.cost[j] = qnan4();
-      a.angle[j] = qnan4();
+      a.cost0[j] = qnan();
+      a.cost[j] = qnan();
+      a.angle[j] = qnan();
     }
     return;
   }
@@ -153,7 +136,7 @@ __global__ void __launch_bounds__(kTrThreads) triangulate_tracks_ragged_kernel(T
     if (i < len) {
       const size_t r = (size_t)b + i;
       const int cm = a.cams[r];
-      ok = (!a.mask || a.mask[r]) && cm >= 0 && cm < a.n_cams && finite4(a.pts[2 * r]) && finite4(a.pts[2 * r + 1]) &&
+      ok = (!a.mask || a.mask[r]) && cm >= 0 && cm < a.n_cams && finite(a.pts[2 * r]) && finite(a.pts[2 * r + 1]) &&
            a.tab[dg::kTrCamStride * (size_t)cm + dg::kTrCamOk] != 0.0;
       a.mask_out[r] = 0;
     }
@@ -211,13 +194,13 @@ __global__ void __launch_bounds__(kTrThreads) triangulate_tracks_ragged_kernel(T
     }
   }
   if (!has_best) {                                   // no model: n < 2 or no valid hypothesis
-    if (lane < 3) a.X_out[3 * (size_t)j + lane] = qnan4();
+    if (lane < 3) a.X_out[3 * (size_t)j + lane] = qnan();
     if (lane == 0) {
       a.n_inliers[j] = 0;
       a.iters[j] = iters;
-      a.cost0[j] = qnan4();
-      a.cost[j] = qnan4();
-      a.angle[j] = qnan4();
+      a.cost0[j] = qnan();
+      a.cost[j] = qnan();
+      a.angle[j] = qnan();
     }
     return;
   }
@@ -304,7 +287,7 @@ __global__ void __launch_bounds__(kTrThreads) triangulate_tracks_ragged_kernel(T
 
 extern "C" {
 
-const char* dgb200_triangulate_last_error(void) { return g_err4; }
+const char* dgb200_triangulate_last_error(void) { return g_err; }
 
 int dgb200_triangulate_tracks_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R,
                                          const double* d_t, const double* d_K, int k_per_camera, int n_cams,
@@ -315,18 +298,18 @@ int dgb200_triangulate_tracks_ragged_dev(const int32_t* d_cams, const double* d_
                                          double* d_cost_out, double* d_angle_out, void* stream) {
   if (!d_R || !d_t || !d_K || !d_offsets || !d_seeds || !d_X_out || !d_n_inliers_out || !d_iters_out ||
       !d_cost0_out || !d_cost_out || !d_angle_out)
-    return fail4(DGB200_E_ARG, "null buffer");
-  if (obs > 0 && (!d_cams || !d_pts || !d_mask_out)) return fail4(DGB200_E_ARG, "null observation buffer");
-  if (n_tracks < 1 || obs < 0 || n_cams < 1) return fail4(DGB200_E_ARG, "need n_tracks >= 1, obs >= 0 and n_cams >= 1");
-  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail4(DGB200_E_ARG, "px_th must be a positive number");
-  if (!(min_angle >= 0.0 && min_angle < M_PI)) return fail4(DGB200_E_ARG, "min_angle must lie in [0, pi)");
-  if (!(conf > 0.0 && conf <= 1.0)) return fail4(DGB200_E_ARG, "conf must lie in (0, 1]");
-  if (max_iters < 1) return fail4(DGB200_E_ARG, "max_iters must be at least 1");
-  if (refine_iters < 0) return fail4(DGB200_E_ARG, "refine_iters must not be negative");
+    return fail(DGB200_E_ARG, "null buffer");
+  if (obs > 0 && (!d_cams || !d_pts || !d_mask_out)) return fail(DGB200_E_ARG, "null observation buffer");
+  if (n_tracks < 1 || obs < 0 || n_cams < 1) return fail(DGB200_E_ARG, "need n_tracks >= 1, obs >= 0 and n_cams >= 1");
+  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail(DGB200_E_ARG, "px_th must be a positive number");
+  if (!(min_angle >= 0.0 && min_angle < M_PI)) return fail(DGB200_E_ARG, "min_angle must lie in [0, pi)");
+  if (!(conf > 0.0 && conf <= 1.0)) return fail(DGB200_E_ARG, "conf must lie in (0, 1]");
+  if (max_iters < 1) return fail(DGB200_E_ARG, "max_iters must be at least 1");
+  if (refine_iters < 0) return fail(DGB200_E_ARG, "refine_iters must not be negative");
   const cudaStream_t st = (cudaStream_t)stream;
   const size_t tab_bytes = sizeof(double) * dg::kTrCamStride * (size_t)n_cams;
   char* ws = nullptr;
-  CU4(cudaMallocAsync((void**)&ws, tab_bytes + sizeof(int) * (size_t)(obs > 0 ? obs : 1), st));
+  CU(cudaMallocAsync((void**)&ws, tab_bytes + sizeof(int) * (size_t)(obs > 0 ? obs : 1), st));
   TriArgs a;
   a.cams = d_cams; a.pts = d_pts; a.tab = (const double*)ws; a.n_cams = n_cams; a.offsets = d_offsets; a.mask = d_mask;
   a.n_tracks = n_tracks; a.obs = obs; a.max_iters = max_iters; a.refine_iters = refine_iters;
@@ -340,8 +323,8 @@ int dgb200_triangulate_tracks_ragged_dev(const int32_t* d_cams, const double* d_
     triangulate_tracks_ragged_kernel<<<(n_tracks + kTrWarps - 1) / kTrWarps, kTrThreads, 0, st>>>(a);
     launch = cudaGetLastError();
   }
-  CU4(cudaFreeAsync(ws, st));
-  CU4(launch);
+  CU(cudaFreeAsync(ws, st));
+  CU(launch);
   return 0;
 }
 

@@ -132,6 +132,141 @@ def _binary_words(descs):
     return rows.view(torch.int32)
 
 
+# ------------------------------------------------------------------------------------------------ argument checks
+# Each helper raises the ValueError of one rule that the entry points share; a wrapper runs them in its own order.
+def _check_tensors(named, mask):
+    """named: (name, value) pairs of the required tensor arguments; mask: the optional one"""
+    import torch
+    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
+        if not isinstance(x, torch.Tensor):
+            raise ValueError("%s must be a torch tensor" % nm)
+
+
+def _check_model(name, M):
+    """a [P,3,3] or [P,9] model tensor; returns P"""
+    if M.dim() not in (2, 3) or M.shape[0] < 1 or tuple(M.shape[1:]) not in ((3, 3), (9,)):
+        raise ValueError("%s must be [P,3,3] or [P,9] with P >= 1, not %s" % (name, list(M.shape)))
+    return int(M.shape[0])
+
+
+def _check_points(pts1, pts2):
+    """the [rows, 2|6] correspondence rows; returns (rows, dim)"""
+    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
+        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
+    return int(pts1.shape[0]), int(pts1.shape[1])
+
+
+def _check_shape(name, x, letter, shape):
+    """x of exactly `shape`, whose first dimension is called `letter` in the message"""
+    if tuple(x.shape) != shape:
+        raise ValueError("%s must be [%s] = [%s], not %s" % (name, ",".join((letter,) + tuple(map(str, shape[1:]))),
+                                                          ",".join(map(str, shape)), list(x.shape)))
+
+
+def _check_columns(name, x, letter, cols):
+    """x of shape [rows, cols], the rows called `letter` in the message; returns rows"""
+    if x.dim() != 2 or x.shape[1] != cols:
+        raise ValueError("%s must be [%s,%d], not %s" % (name, letter, cols, list(x.shape)))
+    return int(x.shape[0])
+
+
+def _check_K(name, K, letter, n):
+    """intrinsics [3,3] shared or [n,3,3], one per pair or camera (`letter`)"""
+    if tuple(K.shape) not in ((3, 3), (n, 3, 3)):
+        raise ValueError("%s must be [3,3] or [%s,3,3] with %s = %d, not %s" % (name, letter, letter, n, list(K.shape)))
+
+
+def _check_int32(name, x):
+    import torch
+    if x.dtype != torch.int32:
+        raise ValueError("%s must be int32, not %s" % (name, x.dtype))
+
+
+def _check_offsets(offsets, letter, n=None):
+    """int32 offsets [n+1] for a given n, or [N+1] with N >= 1 (N called `letter`); returns N"""
+    if n is not None:
+        if tuple(offsets.shape) != (n + 1,):
+            raise ValueError("offsets must be [%s+1] = [%d], not %s" % (letter, n + 1, list(offsets.shape)))
+    elif offsets.dim() != 1 or offsets.shape[0] < 2:
+        raise ValueError("offsets must be [%s+1] with %s >= 1, not %s" % (letter, letter, list(offsets.shape)))
+    _check_int32("offsets", offsets)
+    return int(offsets.shape[0]) - 1
+
+
+def _check_floating(named):
+    for nm, x in named:
+        if not x.is_floating_point():
+            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
+
+
+def _check_mask(mask, letter, rows):
+    """an optional row mask [rows], bool or uint8"""
+    import torch
+    if mask is not None:
+        _check_shape("mask", mask, letter, (rows,))
+        if mask.dtype not in (torch.bool, torch.uint8):
+            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+
+
+def _check_count(name, value, least):
+    """an iteration bound: an int >= least (0 or 1)"""
+    value = int(value)
+    if value < least:
+        raise ValueError("%s must not be negative, not %d" % (name, value) if least == 0 else
+                         "%s must be at least %d, not %d" % (name, least, value))
+    return value
+
+
+def _check_px_th(px_th, positive):
+    """a pixel threshold: finite and > 0 (positive) or >= 0"""
+    px_th = float(px_th)
+    if not (0.0 < px_th < float("inf") if positive else px_th >= 0.0):
+        raise ValueError("px_th must be a %s number, not %r" % ("positive" if positive else "non-negative", px_th))
+    return px_th
+
+
+def _check_conf(conf):
+    conf = float(conf)
+    if not 0.0 < conf <= 1.0:
+        raise ValueError("conf must lie in (0, 1], not %r" % (conf,))
+    return conf
+
+
+def _check_device(named, mask):
+    """the one CUDA device of the tensors of _check_tensors"""
+    dev = named[0][1].device
+    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
+        raise ValueError("%s and mask must be CUDA tensors on one device" % ", ".join(nm for nm, _ in named))
+    return dev
+
+
+def _f64(*xs):
+    import torch
+    return tuple(x.to(torch.float64).contiguous() for x in xs)
+
+
+def _mask_u8(mask):
+    import torch
+    return mask.contiguous().view(torch.uint8) if mask is not None else None
+
+
+def _rows_out(n, dev):
+    """a uint8 row output [n] (never a zero-sized allocation, which would pass a null pointer)"""
+    import torch
+    return torch.empty(max(n, 1), dtype=torch.uint8, device=dev)[:n]
+
+
+def _call(fn, last_error, dev, *args):
+    """fn(*args, stream) on device dev and its current stream, tensors passed by their data pointers and None as a
+    null pointer; a nonzero return code raises ValueError with the message of last_error()"""
+    import torch
+    args = [ctypes.c_void_p(a.data_ptr()) if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        rc = fn(*args, ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+    if rc != 0:
+        raise ValueError(last_error().decode())
+
+
 def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False, norm="l2"):
     """Two-nearest-neighbour matching + SNN ratio test (+ optional mutual nearest-neighbour check).
 
@@ -159,34 +294,25 @@ def match_descriptors(desc1, desc2, kp1=None, kp2=None, ratio=0.9, mutual=False,
     n2 = d2.shape[0]
     dev = d1.device
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        mq = torch.empty(n1, dtype=torch.int32, device=dev)
-        mt = torch.empty(n1, dtype=torch.int32, device=dev)
-        cnt = torch.zeros(1, dtype=torch.int32, device=dev)
-        ws = torch.empty(int(L.dgb200_match_workspace_bytes(n1, n2)), dtype=torch.uint8, device=dev)
-        k1 = k2 = x1 = x2 = None
-        kp_dim = out_dim = 0
-        if kp1 is not None:
-            k1 = kp1.to(device=dev, dtype=torch.float64).contiguous()
-            k2 = kp2.to(device=dev, dtype=torch.float64).contiguous()
-            if k1.shape[0] != n1 or k2.shape[0] != n2 or k1.shape[1] != k2.shape[1] or k1.shape[1] < 2:
-                raise ValueError("keypoint tensors must be [n1,k], [n2,k] with k >= 2")
-            kp_dim = int(k1.shape[1])
-            out_dim = 6 if kp_dim >= 6 else 2
-            x1 = torch.empty((n1, out_dim), dtype=torch.float64, device=dev)
-            x2 = torch.empty((n1, out_dim), dtype=torch.float64, device=dev)
-        stream = torch.cuda.current_stream(dev).cuda_stream
-        vp = ctypes.c_void_p
-        fn, r = ((L.dgb200_match_binary_descriptors_dev, ctypes.c_double(ratio)) if hamming else
-                 (L.dgb200_match_descriptors_dev, ctypes.c_float(ratio)))
-        rc = fn(vp(d1.data_ptr()), n1, vp(d2.data_ptr()), n2, D, r, int(bool(mutual)),
-                vp(k1.data_ptr()) if k1 is not None else None, vp(k2.data_ptr()) if k2 is not None else None, kp_dim,
-                vp(mq.data_ptr()), vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
-                vp(x2.data_ptr()) if x2 is not None else None, out_dim, n1, vp(cnt.data_ptr()), vp(ws.data_ptr()),
-                vp(stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
-        n = int(cnt.item())          # the one host read of the front-end: how many tentatives there are
+    mq = torch.empty(n1, dtype=torch.int32, device=dev)
+    mt = torch.empty(n1, dtype=torch.int32, device=dev)
+    cnt = torch.zeros(1, dtype=torch.int32, device=dev)
+    ws = torch.empty(int(L.dgb200_match_workspace_bytes(n1, n2)), dtype=torch.uint8, device=dev)
+    k1 = k2 = x1 = x2 = None
+    kp_dim = out_dim = 0
+    if kp1 is not None:
+        k1 = kp1.to(device=dev, dtype=torch.float64).contiguous()
+        k2 = kp2.to(device=dev, dtype=torch.float64).contiguous()
+        if k1.shape[0] != n1 or k2.shape[0] != n2 or k1.shape[1] != k2.shape[1] or k1.shape[1] < 2:
+            raise ValueError("keypoint tensors must be [n1,k], [n2,k] with k >= 2")
+        kp_dim = int(k1.shape[1])
+        out_dim = 6 if kp_dim >= 6 else 2
+        x1 = torch.empty((n1, out_dim), dtype=torch.float64, device=dev)
+        x2 = torch.empty((n1, out_dim), dtype=torch.float64, device=dev)
+    fn = L.dgb200_match_binary_descriptors_dev if hamming else L.dgb200_match_descriptors_dev
+    _call(fn, L.dgb200_frontend_last_error, dev, d1, n1, d2, n2, D, ratio, int(bool(mutual)), k1, k2, kp_dim, mq, mt,
+          x1, x2, out_dim, n1, cnt, ws)
+    n = int(cnt.item())          # the one host read of the front-end: how many tentatives there are
     out = (mq[:n].long(), mt[:n].long())
     if x1 is not None:
         out = out + (x1[:n], x2[:n])
@@ -214,61 +340,31 @@ def pose_from_fundamental(F, K1, K2, pts1, pts2, mask=None):
     if mask is not None:
         m = mask.to(device=dev, dtype=torch.uint8).contiguous()
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        R = torch.empty((P, 3, 3), dtype=torch.float64, device=dev)
-        t = torch.empty((P, 3), dtype=torch.float64, device=dev)
-        good = torch.empty(P, dtype=torch.int32, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_pose_from_fundamental_batch_dev(vp(Fc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), per_pair,
-                                                      vp(p1.data_ptr()), vp(p2.data_ptr()),
-                                                      vp(m.data_ptr()) if m is not None else None, P, N, dim,
-                                                      vp(R.data_ptr()), vp(t.data_ptr()), vp(good.data_ptr()),
-                                                      vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    R = torch.empty((P, 3, 3), dtype=torch.float64, device=dev)
+    t = torch.empty((P, 3), dtype=torch.float64, device=dev)
+    good = torch.empty(P, dtype=torch.int32, device=dev)
+    _call(L.dgb200_pose_from_fundamental_batch_dev, L.dgb200_frontend_last_error, dev, Fc, K1c, K2c, per_pair, p1, p2,
+          m, P, N, dim, R, t, good)
     return R, t, good
 
 
 def _ragged_pose_inputs(model, name, K1, K2, pts1, pts2, offsets, mask):
     """Checks the inputs of a ragged pose call (a [P,3,3] or [P,9] model named `name`, K, rows, offsets, mask) and returns
     them ready for the C ABI: (P, rows, dim, device, per_pair, model, K1, K2, pts1, pts2, offsets, mask or None)."""
-    import torch
     named = ((name, model), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
-    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % nm)
-    if model.dim() not in (2, 3) or model.shape[0] < 1 or tuple(model.shape[1:]) not in ((3, 3), (9,)):
-        raise ValueError("%s must be [P,3,3] or [P,9] with P >= 1, not %s" % (name, list(model.shape)))
-    P = int(model.shape[0])
-    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
-        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
-    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
-    for nm, K in (("K1", K1), ("K2", K2)):
-        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
-            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (nm, P, list(K.shape)))
-    if tuple(offsets.shape) != (P + 1,):
-        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
-    if offsets.dtype != torch.int32:
-        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    for nm, x in ((name, model), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (rows,):
-            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    dev = pts1.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("%s, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device" % name)
+    _check_tensors(named, mask)
+    P = _check_model(name, model)
+    rows, dim = _check_points(pts1, pts2)
+    _check_K("K1", K1, "P", P)
+    _check_K("K2", K2, "P", P)
+    _check_offsets(offsets, "P", P)
+    _check_floating(named[:5])
+    _check_mask(mask, "rows", rows)
+    dev = _check_device(named, mask)
     per_pair = K1.dim() == 3 or K2.dim() == 3
     if per_pair:
         K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
-    f64 = torch.float64
-    Mc, K1c, K2c = (x.to(f64).contiguous() for x in (model, K1, K2))
-    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
-    return P, rows, dim, dev, int(per_pair), Mc, K1c, K2c, p1, p2, offsets.contiguous(), m
+    return (P, rows, dim, dev, int(per_pair)) + _f64(model, K1, K2, pts1, pts2) + (offsets.contiguous(), _mask_u8(mask))
 
 
 def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
@@ -290,22 +386,15 @@ def pose_from_fundamental_ragged(F, K1, K2, pts1, pts2, offsets, mask=None):
                                                                                     offsets, mask)
     f64 = torch.float64
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        R = torch.empty((P, 3, 3), dtype=f64, device=dev)
-        t = torch.empty((P, 3), dtype=f64, device=dev)
-        good = torch.empty(P, dtype=torch.int32, device=dev)
-        points = torch.empty((rows, 3), dtype=f64, device=dev)
-        in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
-        angle = torch.empty(rows, dtype=f64, device=dev)
-        median = torch.empty(P, dtype=f64, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_pose_from_fundamental_ragged_dev(
-            vp(Fc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), per_pair, vp(p1.data_ptr()),
-            vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim, vp(m.data_ptr()) if m is not None else None,
-            vp(R.data_ptr()), vp(t.data_ptr()), vp(good.data_ptr()), vp(points.data_ptr()), vp(in_front.data_ptr()),
-            vp(angle.data_ptr()), vp(median.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    R = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    t = torch.empty((P, 3), dtype=f64, device=dev)
+    good = torch.empty(P, dtype=torch.int32, device=dev)
+    points = torch.empty((rows, 3), dtype=f64, device=dev)
+    in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
+    angle = torch.empty(rows, dtype=f64, device=dev)
+    median = torch.empty(P, dtype=f64, device=dev)
+    _call(L.dgb200_pose_from_fundamental_ragged_dev, L.dgb200_frontend_last_error, dev, Fc, K1c, K2c, per_pair, p1,
+          p2, off, P, rows, dim, m, R, t, good, points, in_front, angle, median)
     return RaggedPose(R, t, good, points, in_front.view(torch.bool), angle, median)
 
 
@@ -336,25 +425,17 @@ def pose_from_homography_ragged(H, K1, K2, pts1, pts2, offsets, mask=None):
                                                                                     offsets, mask)
     f64 = torch.float64
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        R = torch.empty((P, 2, 3, 3), dtype=f64, device=dev)
-        t = torch.empty((P, 2, 3), dtype=f64, device=dev)
-        plane = torch.empty((P, 2, 4), dtype=f64, device=dev)
-        good = torch.empty((P, 2), dtype=torch.int32, device=dev)
-        rotation_only = torch.empty(P, dtype=torch.uint8, device=dev)
-        points = torch.empty((rows, 3), dtype=f64, device=dev)
-        in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
-        angle = torch.empty(rows, dtype=f64, device=dev)
-        median = torch.empty(P, dtype=f64, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_pose_from_homography_ragged_dev(
-            vp(Hc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), per_pair, vp(p1.data_ptr()),
-            vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim, vp(m.data_ptr()) if m is not None else None,
-            vp(R.data_ptr()), vp(t.data_ptr()), vp(plane.data_ptr()), vp(good.data_ptr()), vp(rotation_only.data_ptr()),
-            vp(points.data_ptr()), vp(in_front.data_ptr()), vp(angle.data_ptr()), vp(median.data_ptr()),
-            vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    R = torch.empty((P, 2, 3, 3), dtype=f64, device=dev)
+    t = torch.empty((P, 2, 3), dtype=f64, device=dev)
+    plane = torch.empty((P, 2, 4), dtype=f64, device=dev)
+    good = torch.empty((P, 2), dtype=torch.int32, device=dev)
+    rotation_only = torch.empty(P, dtype=torch.uint8, device=dev)
+    points = torch.empty((rows, 3), dtype=f64, device=dev)
+    in_front = torch.empty(rows, dtype=torch.uint8, device=dev)
+    angle = torch.empty(rows, dtype=f64, device=dev)
+    median = torch.empty(P, dtype=f64, device=dev)
+    _call(L.dgb200_pose_from_homography_ragged_dev, L.dgb200_frontend_last_error, dev, Hc, K1c, K2c, per_pair, p1,
+          p2, off, P, rows, dim, m, R, t, plane, good, rotation_only, points, in_front, angle, median)
     return HomographyPose(R, t, plane, good, rotation_only.view(torch.bool), points, in_front.view(torch.bool), angle,
                           median)
 
@@ -379,70 +460,37 @@ def refine_pose_ragged(R, t, K1, K2, pts1, pts2, offsets, mask=None, max_iters=1
     no inliers.  The result of a pair does not depend on the batch it is in.  Asynchronous, nothing is read back."""
     import torch
     named = (("R", R), ("t", t), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
-    for name, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % name)
-    if R.dim() not in (2, 3) or R.shape[0] < 1 or tuple(R.shape[1:]) not in ((3, 3), (9,)):
-        raise ValueError("R must be [P,3,3] or [P,9] with P >= 1, not %s" % list(R.shape))
-    P = int(R.shape[0])
-    if tuple(t.shape) != (P, 3):
-        raise ValueError("t must be [P,3] = [%d,3], not %s" % (P, list(t.shape)))
-    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
-        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
-    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
-    for name, K in (("K1", K1), ("K2", K2)):
-        if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
-            raise ValueError("%s must be [3,3] or [P,3,3] with P = %d, not %s" % (name, P, list(K.shape)))
-    if tuple(offsets.shape) != (P + 1,):
-        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
-    if offsets.dtype != torch.int32:
-        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    for name, x in (("R", R), ("t", t), ("K1", K1), ("K2", K2), ("pts1", pts1), ("pts2", pts2)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (name, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (rows,):
-            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    max_iters = int(max_iters)
-    if max_iters < 0:
-        raise ValueError("max_iters must not be negative, not %d" % max_iters)
+    _check_tensors(named, mask)
+    P = _check_model("R", R)
+    _check_shape("t", t, "P", (P, 3))
+    rows, dim = _check_points(pts1, pts2)
+    _check_K("K1", K1, "P", P)
+    _check_K("K2", K2, "P", P)
+    _check_offsets(offsets, "P", P)
+    _check_floating(named[:6])
+    _check_mask(mask, "rows", rows)
+    max_iters = _check_count("max_iters", max_iters, 0)
     if px_th is not None:
-        px_th = float(px_th)
-        if not px_th >= 0.0:
-            raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
-    dev = pts1.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("R, t, K1, K2, pts1, pts2, offsets and mask must be CUDA tensors on one device")
+        px_th = _check_px_th(px_th, False)
+    dev = _check_device(named, mask)
     per_pair = K1.dim() == 3 or K2.dim() == 3
     if per_pair:
         K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    Rc, tc, K1c, K2c, p1, p2 = _f64(R, t, K1, K2, pts1, pts2)
+    off, m = offsets.contiguous(), _mask_u8(mask)
     f64 = torch.float64
-    Rc, tc, K1c, K2c = (x.to(f64).contiguous() for x in (R, t, K1, K2))
-    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
-    off = offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        Ro = torch.empty((P, 3, 3), dtype=f64, device=dev)
-        to = torch.empty((P, 3), dtype=f64, device=dev)
-        Fo = torch.empty((P, 3, 3), dtype=f64, device=dev)
-        cost0 = torch.empty(P, dtype=f64, device=dev)
-        cost = torch.empty(P, dtype=f64, device=dev)
-        n_used = torch.empty(P, dtype=torch.int32, device=dev)
-        iters = torch.empty(P, dtype=torch.int32, device=dev)
-        inl = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows] if px_th is not None else None
-        vp = ctypes.c_void_p
-        rc = L.dgb200_refine_pose_ragged_dev(
-            vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(K1c.data_ptr()), vp(K2c.data_ptr()), int(per_pair),
-            vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
-            vp(m.data_ptr()) if m is not None else None, max_iters, ctypes.c_double(px_th if px_th is not None else 0.0),
-            vp(Ro.data_ptr()), vp(to.data_ptr()), vp(Fo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()),
-            vp(n_used.data_ptr()), vp(iters.data_ptr()), vp(inl.data_ptr()) if inl is not None else None,
-            vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    Ro = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    to = torch.empty((P, 3), dtype=f64, device=dev)
+    Fo = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    cost0 = torch.empty(P, dtype=f64, device=dev)
+    cost = torch.empty(P, dtype=f64, device=dev)
+    n_used = torch.empty(P, dtype=torch.int32, device=dev)
+    iters = torch.empty(P, dtype=torch.int32, device=dev)
+    inl = _rows_out(rows, dev) if px_th is not None else None
+    _call(L.dgb200_refine_pose_ragged_dev, L.dgb200_frontend_last_error, dev, Rc, tc, K1c, K2c, int(per_pair), p1, p2,
+          off, P, rows, dim, m, max_iters, px_th if px_th is not None else 0.0, Ro, to, Fo, cost0, cost, n_used, iters,
+          inl)
     return RefinedPose(Ro, to, Fo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None)
 
 
@@ -500,58 +548,28 @@ def _refine_model_ragged(name, entry, M, pts1, pts2, offsets, mask, max_iters, p
     point `entry`: the refined models [P,3,3], cost0, cost, n_used, iters and the inlier rows (None without px_th)."""
     import torch
     named = ((name, M), ("pts1", pts1), ("pts2", pts2), ("offsets", offsets))
-    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % nm)
-    if M.dim() not in (2, 3) or M.shape[0] < 1 or tuple(M.shape[1:]) not in ((3, 3), (9,)):
-        raise ValueError("%s must be [P,3,3] or [P,9] with P >= 1, not %s" % (name, list(M.shape)))
-    P = int(M.shape[0])
-    if pts1.dim() != 2 or pts1.shape[1] < 2 or pts2.shape != pts1.shape:
-        raise ValueError("pts1 and pts2 must be [rows, 2|6] tensors of one shape")
-    rows, dim = int(pts1.shape[0]), int(pts1.shape[1])
-    if tuple(offsets.shape) != (P + 1,):
-        raise ValueError("offsets must be [P+1] = [%d], not %s" % (P + 1, list(offsets.shape)))
-    if offsets.dtype != torch.int32:
-        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    for nm, x in ((name, M), ("pts1", pts1), ("pts2", pts2)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (rows,):
-            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    max_iters = int(max_iters)
-    if max_iters < 0:
-        raise ValueError("max_iters must not be negative, not %d" % max_iters)
+    _check_tensors(named, mask)
+    P = _check_model(name, M)
+    rows, dim = _check_points(pts1, pts2)
+    _check_offsets(offsets, "P", P)
+    _check_floating(named[:3])
+    _check_mask(mask, "rows", rows)
+    max_iters = _check_count("max_iters", max_iters, 0)
     if px_th is not None:
-        px_th = float(px_th)
-        if not px_th >= 0.0:
-            raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
-    dev = pts1.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("%s, pts1, pts2, offsets and mask must be CUDA tensors on one device" % name)
+        px_th = _check_px_th(px_th, False)
+    dev = _check_device(named, mask)
+    Mc, p1, p2 = _f64(M, pts1, pts2)
+    off, m = offsets.contiguous(), _mask_u8(mask)
     f64 = torch.float64
-    Mc = M.to(f64).contiguous()
-    p1, p2 = pts1.to(f64).contiguous(), pts2.to(f64).contiguous()
-    off = offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        Mo = torch.empty((P, 3, 3), dtype=f64, device=dev)
-        cost0 = torch.empty(P, dtype=f64, device=dev)
-        cost = torch.empty(P, dtype=f64, device=dev)
-        n_used = torch.empty(P, dtype=torch.int32, device=dev)
-        iters = torch.empty(P, dtype=torch.int32, device=dev)
-        inl = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows] if px_th is not None else None
-        vp = ctypes.c_void_p
-        rc = getattr(L, entry)(
-            vp(Mc.data_ptr()), vp(p1.data_ptr()), vp(p2.data_ptr()), vp(off.data_ptr()), P, rows, dim,
-            vp(m.data_ptr()) if m is not None else None, max_iters, ctypes.c_double(px_th if px_th is not None else 0.0),
-            vp(Mo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(n_used.data_ptr()), vp(iters.data_ptr()),
-            vp(inl.data_ptr()) if inl is not None else None, vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    Mo = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    cost0 = torch.empty(P, dtype=f64, device=dev)
+    cost = torch.empty(P, dtype=f64, device=dev)
+    n_used = torch.empty(P, dtype=torch.int32, device=dev)
+    iters = torch.empty(P, dtype=torch.int32, device=dev)
+    inl = _rows_out(rows, dev) if px_th is not None else None
+    _call(getattr(L, entry), L.dgb200_frontend_last_error, dev, Mc, p1, p2, off, P, rows, dim, m, max_iters,
+          px_th if px_th is not None else 0.0, Mo, cost0, cost, n_used, iters, inl)
     return Mo, cost0, cost, n_used, iters, inl.view(torch.bool) if inl is not None else None
 
 
@@ -578,70 +596,51 @@ def find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=None, px_th=2.0, co
     import torch
     from .tensor_api import _seeds_tensor
     named = (("pts2d", pts2d), ("pts3d", pts3d), ("K", K), ("offsets", offsets))
-    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % nm)
-    if offsets.dim() != 1 or offsets.shape[0] < 2:
-        raise ValueError("offsets must be [P+1] with P >= 1, not %s" % list(offsets.shape))
-    if offsets.dtype != torch.int32:
-        raise ValueError("offsets must be int32, not %s" % offsets.dtype)
-    P = int(offsets.shape[0]) - 1
-    if pts2d.dim() != 2 or pts2d.shape[1] != 2:
-        raise ValueError("pts2d must be [rows,2], not %s" % list(pts2d.shape))
-    rows = int(pts2d.shape[0])
-    if tuple(pts3d.shape) != (rows, 3):
-        raise ValueError("pts3d must be [rows,3] = [%d,3], not %s" % (rows, list(pts3d.shape)))
-    if tuple(K.shape) not in ((3, 3), (P, 3, 3)):
-        raise ValueError("K must be [3,3] or [P,3,3] with P = %d, not %s" % (P, list(K.shape)))
-    for nm, x in (("pts2d", pts2d), ("pts3d", pts3d), ("K", K)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (rows,):
-            raise ValueError("mask must be [rows] = [%d], not %s" % (rows, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    px_th, conf = float(px_th), float(conf)
-    if not 0.0 < px_th < float("inf"):
-        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
-    if not 0.0 < conf <= 1.0:
-        raise ValueError("conf must lie in (0, 1], not %r" % (conf,))
-    max_iters, refine_iters = int(max_iters), int(refine_iters)
-    if max_iters < 1:
-        raise ValueError("max_iters must be at least 1, not %d" % max_iters)
-    if refine_iters < 0:
-        raise ValueError("refine_iters must not be negative, not %d" % refine_iters)
-    dev = pts2d.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("pts2d, pts3d, K, offsets and mask must be CUDA tensors on one device")
+    _check_tensors(named, mask)
+    P = _check_offsets(offsets, "P")
+    rows = _check_columns("pts2d", pts2d, "rows", 2)
+    _check_shape("pts3d", pts3d, "rows", (rows, 3))
+    _check_K("K", K, "P", P)
+    _check_floating(named[:3])
+    _check_mask(mask, "rows", rows)
+    px_th = _check_px_th(px_th, True)
+    conf = _check_conf(conf)
+    max_iters = _check_count("max_iters", max_iters, 1)
+    refine_iters = _check_count("refine_iters", refine_iters, 0)
+    dev = _check_device(named, mask)
     if isinstance(seeds, torch.Tensor) and seeds.is_cuda and seeds.device != dev:
         raise ValueError("seeds must be on the device of pts2d")
+    x, X, Kc = _f64(pts2d, pts3d, K)
+    off, m = offsets.contiguous(), _mask_u8(mask)
+    ds = _seeds_tensor(seeds, P, dev)
+    if tuple(ds.shape) != (P,):
+        raise ValueError("seeds must hold one seed per pair (%d), not %s" % (P, list(ds.shape)))
     f64 = torch.float64
-    x, X, Kc = pts2d.to(f64).contiguous(), pts3d.to(f64).contiguous(), K.to(f64).contiguous()
-    off = offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        ds = _seeds_tensor(seeds, P, dev)
-        if tuple(ds.shape) != (P,):
-            raise ValueError("seeds must hold one seed per pair (%d), not %s" % (P, list(ds.shape)))
-        R = torch.empty((P, 3, 3), dtype=f64, device=dev)
-        t = torch.empty((P, 3), dtype=f64, device=dev)
-        mo = torch.empty(max(rows, 1), dtype=torch.uint8, device=dev)[:rows]
-        n_inl = torch.empty(P, dtype=torch.int32, device=dev)
-        iters = torch.empty(P, dtype=torch.int32, device=dev)
-        cost0 = torch.empty(P, dtype=f64, device=dev)
-        cost = torch.empty(P, dtype=f64, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_find_absolute_pose_ragged_dev(
-            vp(x.data_ptr()), vp(X.data_ptr()), vp(Kc.data_ptr()), int(Kc.dim() == 3), vp(off.data_ptr()), P, rows,
-            vp(m.data_ptr()) if m is not None else None, ctypes.c_double(px_th), ctypes.c_double(conf), max_iters,
-            refine_iters, vp(ds.data_ptr()), vp(R.data_ptr()), vp(t.data_ptr()), vp(mo.data_ptr()),
-            vp(n_inl.data_ptr()), vp(iters.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()),
-            vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_absolute_pose_last_error().decode())
+    R = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    t = torch.empty((P, 3), dtype=f64, device=dev)
+    mo = _rows_out(rows, dev)
+    n_inl = torch.empty(P, dtype=torch.int32, device=dev)
+    iters = torch.empty(P, dtype=torch.int32, device=dev)
+    cost0 = torch.empty(P, dtype=f64, device=dev)
+    cost = torch.empty(P, dtype=f64, device=dev)
+    _call(L.dgb200_find_absolute_pose_ragged_dev, L.dgb200_absolute_pose_last_error, dev, x, X, Kc, int(Kc.dim() == 3),
+          off, P, rows, m, px_th, conf, max_iters, refine_iters, ds, R, t, mo, n_inl, iters, cost0, cost)
     return AbsolutePose(R, t, mo.view(torch.bool), n_inl, iters, cost0, cost)
+
+
+def _check_tracks(cams, pts, R, t, K, offsets):
+    """the track layout of triangulate_tracks_ragged and bundle_adjust_ragged; returns (T, obs, C)"""
+    T = _check_offsets(offsets, "T")
+    _check_int32("cams", cams)
+    obs = _check_columns("pts", pts, "obs", 2)
+    _check_shape("cams", cams, "obs", (obs,))
+    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
+        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
+    C = int(R.shape[0])
+    _check_shape("t", t, "C", (C, 3))
+    _check_K("K", K, "C", C)
+    return T, obs, C
 
 
 def triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=None, px_th=2.0, min_angle=math.radians(1.5),
@@ -670,77 +669,36 @@ def triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=None, px_th=2.0,
     import torch
     from .tensor_api import _seeds_tensor
     named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("K", K), ("offsets", offsets))
-    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % nm)
-    if offsets.dim() != 1 or offsets.shape[0] < 2:
-        raise ValueError("offsets must be [T+1] with T >= 1, not %s" % list(offsets.shape))
-    for nm, x in (("offsets", offsets), ("cams", cams)):
-        if x.dtype != torch.int32:
-            raise ValueError("%s must be int32, not %s" % (nm, x.dtype))
-    T = int(offsets.shape[0]) - 1
-    if pts.dim() != 2 or pts.shape[1] != 2:
-        raise ValueError("pts must be [obs,2], not %s" % list(pts.shape))
-    obs = int(pts.shape[0])
-    if tuple(cams.shape) != (obs,):
-        raise ValueError("cams must be [obs] = [%d], not %s" % (obs, list(cams.shape)))
-    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
-        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
-    C = int(R.shape[0])
-    if tuple(t.shape) != (C, 3):
-        raise ValueError("t must be [C,3] = [%d,3], not %s" % (C, list(t.shape)))
-    if tuple(K.shape) not in ((3, 3), (C, 3, 3)):
-        raise ValueError("K must be [3,3] or [C,3,3] with C = %d, not %s" % (C, list(K.shape)))
-    for nm, x in (("pts", pts), ("R", R), ("t", t), ("K", K)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (obs,):
-            raise ValueError("mask must be [obs] = [%d], not %s" % (obs, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
-    px_th, min_angle, conf = float(px_th), float(min_angle), float(conf)
-    if not 0.0 < px_th < float("inf"):
-        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
+    _check_tensors(named, mask)
+    T, obs, C = _check_tracks(cams, pts, R, t, K, offsets)
+    _check_floating(named[1:5])
+    _check_mask(mask, "obs", obs)
+    px_th, min_angle = _check_px_th(px_th, True), float(min_angle)
     if not 0.0 <= min_angle < math.pi:
         raise ValueError("min_angle must lie in [0, pi), not %r" % (min_angle,))
-    if not 0.0 < conf <= 1.0:
-        raise ValueError("conf must lie in (0, 1], not %r" % (conf,))
-    max_iters, refine_iters = int(max_iters), int(refine_iters)
-    if max_iters < 1:
-        raise ValueError("max_iters must be at least 1, not %d" % max_iters)
-    if refine_iters < 0:
-        raise ValueError("refine_iters must not be negative, not %d" % refine_iters)
-    dev = pts.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("cams, pts, R, t, K, offsets and mask must be CUDA tensors on one device")
+    conf = _check_conf(conf)
+    max_iters = _check_count("max_iters", max_iters, 1)
+    refine_iters = _check_count("refine_iters", refine_iters, 0)
+    dev = _check_device(named, mask)
     if isinstance(seeds, torch.Tensor) and seeds.is_cuda and seeds.device != dev:
         raise ValueError("seeds must be on the device of pts")
+    x, Rc, tc, Kc = _f64(pts, R, t, K)
+    cm, off, m = cams.contiguous(), offsets.contiguous(), _mask_u8(mask)
+    ds = _seeds_tensor(seeds, T, dev)
+    if tuple(ds.shape) != (T,):
+        raise ValueError("seeds must hold one seed per track (%d), not %s" % (T, list(ds.shape)))
     f64 = torch.float64
-    x, Rc, tc, Kc = (v.to(f64).contiguous() for v in (pts, R, t, K))
-    cm, off = cams.contiguous(), offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        ds = _seeds_tensor(seeds, T, dev)
-        if tuple(ds.shape) != (T,):
-            raise ValueError("seeds must hold one seed per track (%d), not %s" % (T, list(ds.shape)))
-        X = torch.empty((T, 3), dtype=f64, device=dev)
-        mo = torch.empty(max(obs, 1), dtype=torch.uint8, device=dev)[:obs]
-        n_inl = torch.empty(T, dtype=torch.int32, device=dev)
-        iters = torch.empty(T, dtype=torch.int32, device=dev)
-        cost0 = torch.empty(T, dtype=f64, device=dev)
-        cost = torch.empty(T, dtype=f64, device=dev)
-        angle = torch.empty(T, dtype=f64, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_triangulate_tracks_ragged_dev(
-            vp(cm.data_ptr()), vp(x.data_ptr()), vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(Kc.data_ptr()),
-            int(Kc.dim() == 3), C, vp(off.data_ptr()), T, obs, vp(m.data_ptr()) if m is not None else None,
-            ctypes.c_double(px_th), ctypes.c_double(min_angle), ctypes.c_double(conf), max_iters, refine_iters,
-            vp(ds.data_ptr()), vp(X.data_ptr()), vp(mo.data_ptr()), vp(n_inl.data_ptr()), vp(iters.data_ptr()),
-            vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(angle.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_triangulate_last_error().decode())
+    X = torch.empty((T, 3), dtype=f64, device=dev)
+    mo = _rows_out(obs, dev)
+    n_inl = torch.empty(T, dtype=torch.int32, device=dev)
+    iters = torch.empty(T, dtype=torch.int32, device=dev)
+    cost0 = torch.empty(T, dtype=f64, device=dev)
+    cost = torch.empty(T, dtype=f64, device=dev)
+    angle = torch.empty(T, dtype=f64, device=dev)
+    _call(L.dgb200_triangulate_tracks_ragged_dev, L.dgb200_triangulate_last_error, dev, cm, x, Rc, tc, Kc,
+          int(Kc.dim() == 3), C, off, T, obs, m, px_th, min_angle, conf, max_iters, refine_iters, ds, X, mo, n_inl,
+          iters, cost0, cost, angle)
     return Tracks(X, mo.view(torch.bool), n_inl, iters, cost0, cost, angle)
 
 
@@ -772,37 +730,11 @@ def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, s
     trial steps; n_used: [1] int32 the observations in the cost.  Asynchronous, nothing is read back."""
     import torch
     named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("K", K), ("offsets", offsets), ("X", X))
-    for nm, x in named + ((("mask", mask),) if mask is not None else ()):
-        if not isinstance(x, torch.Tensor):
-            raise ValueError("%s must be a torch tensor" % nm)
-    if offsets.dim() != 1 or offsets.shape[0] < 2:
-        raise ValueError("offsets must be [T+1] with T >= 1, not %s" % list(offsets.shape))
-    for nm, x in (("offsets", offsets), ("cams", cams)):
-        if x.dtype != torch.int32:
-            raise ValueError("%s must be int32, not %s" % (nm, x.dtype))
-    T = int(offsets.shape[0]) - 1
-    if pts.dim() != 2 or pts.shape[1] != 2:
-        raise ValueError("pts must be [obs,2], not %s" % list(pts.shape))
-    obs = int(pts.shape[0])
-    if tuple(cams.shape) != (obs,):
-        raise ValueError("cams must be [obs] = [%d], not %s" % (obs, list(cams.shape)))
-    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
-        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
-    C = int(R.shape[0])
-    if tuple(t.shape) != (C, 3):
-        raise ValueError("t must be [C,3] = [%d,3], not %s" % (C, list(t.shape)))
-    if tuple(K.shape) not in ((3, 3), (C, 3, 3)):
-        raise ValueError("K must be [3,3] or [C,3,3] with C = %d, not %s" % (C, list(K.shape)))
-    if tuple(X.shape) != (T, 3):
-        raise ValueError("X must be [T,3] = [%d,3], not %s" % (T, list(X.shape)))
-    for nm, x in (("pts", pts), ("R", R), ("t", t), ("K", K), ("X", X)):
-        if not x.is_floating_point():
-            raise ValueError("%s must be a floating tensor, not %s" % (nm, x.dtype))
-    if mask is not None:
-        if tuple(mask.shape) != (obs,):
-            raise ValueError("mask must be [obs] = [%d], not %s" % (obs, list(mask.shape)))
-        if mask.dtype not in (torch.bool, torch.uint8):
-            raise ValueError("mask must be bool or uint8, not %s" % mask.dtype)
+    _check_tensors(named, mask)
+    T, obs, C = _check_tracks(cams, pts, R, t, K, offsets)
+    _check_shape("X", X, "T", (T, 3))
+    _check_floating(named[1:5] + named[6:])
+    _check_mask(mask, "obs", obs)
     if free is None:
         if C - 1 > BA_MAX_FREE:
             raise ValueError("free=None frees %d cameras, more than %d: pass an explicit free list" % (C - 1, BA_MAX_FREE))
@@ -837,39 +769,25 @@ def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, s
         sigma = float(loss_scale)
         if not 0.0 < sigma < float("inf"):
             raise ValueError("loss_scale must be a positive number or None, not %r" % (loss_scale,))
-    max_iters, px_th = int(max_iters), float(px_th)
-    if max_iters < 0:
-        raise ValueError("max_iters must not be negative, not %d" % max_iters)
-    if not 0.0 < px_th < float("inf"):
-        raise ValueError("px_th must be a positive number, not %r" % (px_th,))
-    dev = pts.device
-    if dev.type != "cuda" or any(x.device != dev for _, x in named) or (mask is not None and mask.device != dev):
-        raise ValueError("cams, pts, R, t, K, offsets, X and mask must be CUDA tensors on one device")
-    f64 = torch.float64
-    x, Rc, tc, Kc, Xc = (v.to(f64).contiguous() for v in (pts, R, t, K, X))
-    cm, off = cams.contiguous(), offsets.contiguous()
-    m = mask.contiguous().view(torch.uint8) if mask is not None else None
+    max_iters = _check_count("max_iters", max_iters, 0)
+    px_th = _check_px_th(px_th, True)
+    dev = _check_device(named, mask)
+    x, Rc, tc, Kc, Xc = _f64(pts, R, t, K, X)
+    cm, off, m = cams.contiguous(), offsets.contiguous(), _mask_u8(mask)
     hf = np.ascontiguousarray(fr, dtype=np.int32)
+    f64 = torch.float64
     L = _cabi.lib()
-    with torch.cuda.device(dev):
-        Ro = torch.empty((C, 3, 3), dtype=f64, device=dev)
-        to = torch.empty((C, 3), dtype=f64, device=dev)
-        Xo = torch.empty((T, 3), dtype=f64, device=dev)
-        mo = torch.empty(max(obs, 1), dtype=torch.uint8, device=dev)[:obs]
-        cost0 = torch.empty(1, dtype=f64, device=dev)
-        cost = torch.empty(1, dtype=f64, device=dev)
-        iters = torch.empty(1, dtype=torch.int32, device=dev)
-        n_used = torch.empty(1, dtype=torch.int32, device=dev)
-        vp = ctypes.c_void_p
-        rc = L.dgb200_bundle_adjust_ragged_dev(
-            vp(cm.data_ptr()), vp(x.data_ptr()), vp(Rc.data_ptr()), vp(tc.data_ptr()), vp(Kc.data_ptr()),
-            int(Kc.dim() == 3), C, vp(off.data_ptr()), T, obs, vp(Xc.data_ptr()),
-            vp(m.data_ptr()) if m is not None else None, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr),
-            gauge, ctypes.c_double(sigma), max_iters, ctypes.c_double(px_th), vp(Ro.data_ptr()), vp(to.data_ptr()),
-            vp(Xo.data_ptr()), vp(mo.data_ptr()), vp(cost0.data_ptr()), vp(cost.data_ptr()), vp(iters.data_ptr()),
-            vp(n_used.data_ptr()), vp(torch.cuda.current_stream(dev).cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_bundle_adjust_last_error().decode())
+    Ro = torch.empty((C, 3, 3), dtype=f64, device=dev)
+    to = torch.empty((C, 3), dtype=f64, device=dev)
+    Xo = torch.empty((T, 3), dtype=f64, device=dev)
+    mo = _rows_out(obs, dev)
+    cost0 = torch.empty(1, dtype=f64, device=dev)
+    cost = torch.empty(1, dtype=f64, device=dev)
+    iters = torch.empty(1, dtype=torch.int32, device=dev)
+    n_used = torch.empty(1, dtype=torch.int32, device=dev)
+    _call(L.dgb200_bundle_adjust_ragged_dev, L.dgb200_bundle_adjust_last_error, dev, cm, x, Rc, tc, Kc,
+          int(Kc.dim() == 3), C, off, T, obs, Xc, m, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr), gauge,
+          sigma, max_iters, px_th, Ro, to, Xo, mo, cost0, cost, iters, n_used)
     return BundleAdjustment(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used)
 
 
@@ -912,9 +830,7 @@ def match_descriptors_guided(descs, pairs, kps, models, px_th, guide="F", ratio=
     import torch
     if guide not in ("F", "H"):
         raise ValueError("guide must be 'F' or 'H', not %r" % (guide,))
-    px_th = float(px_th)
-    if not px_th >= 0.0:
-        raise ValueError("px_th must be a non-negative number, not %r" % (px_th,))
+    px_th = _check_px_th(px_th, False)
     hamming = _check_norm(norm)
     pairs = _host_pairs(pairs)
     if kps is None:
@@ -986,35 +902,26 @@ def _match_bank(bank, counts, pairs, kbank, ratio, mutual, hamming=False, guide=
     L = _cabi.lib()
     i32 = ctypes.POINTER(ctypes.c_int32)
     cap = max(lay.capacity, 1)        # (a zero-sized allocation would pass a null pointer)
-    with torch.cuda.device(dev):
-        mq = torch.empty(cap, dtype=torch.int32, device=dev)
-        mt = torch.empty(cap, dtype=torch.int32, device=dev)
-        offsets = torch.empty(P + 1, dtype=torch.int32, device=dev)
-        ws = torch.empty(max(int(L.dgb200_match_batch_workspace_bytes(off.ctypes.data_as(i32), len(counts),
-                                                                      pr.ctypes.data_as(i32), P)), 1),
-                         dtype=torch.uint8, device=dev)
-        x1 = x2 = None
-        kp_dim = out_dim = 0
-        if kbank is not None:
-            kp_dim = int(kbank.shape[1])
-            out_dim = 6 if kp_dim >= 6 else 2
-            x1 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
-            x2 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
-        stream = torch.cuda.current_stream(dev)
-        vp = ctypes.c_void_p
-        r = ctypes.c_double(ratio) if hamming else ctypes.c_float(ratio)
-        guided = ()
-        if guide is None:
-            fn = L.dgb200_match_binary_descriptors_batch_dev if hamming else L.dgb200_match_descriptors_batch_dev
-        else:
-            fn = (L.dgb200_match_binary_descriptors_guided_batch_dev if hamming else
-                  L.dgb200_match_descriptors_guided_batch_dev)
-            guided = (vp(models.data_ptr()), int(guide), ctypes.c_double(px_th))
-        rc = fn(vp(bank.data_ptr()), off.ctypes.data_as(i32), len(counts), D, pr.ctypes.data_as(i32), P, *guided, r,
-                int(bool(mutual)), vp(kbank.data_ptr()) if kbank is not None else None, kp_dim, vp(mq.data_ptr()),
-                vp(mt.data_ptr()), vp(x1.data_ptr()) if x1 is not None else None,
-                vp(x2.data_ptr()) if x2 is not None else None, out_dim, cap, vp(offsets.data_ptr()), vp(ws.data_ptr()),
-                vp(stream.cuda_stream))
-        if rc != 0:
-            raise ValueError(L.dgb200_frontend_last_error().decode())
+    mq = torch.empty(cap, dtype=torch.int32, device=dev)
+    mt = torch.empty(cap, dtype=torch.int32, device=dev)
+    offsets = torch.empty(P + 1, dtype=torch.int32, device=dev)
+    ws = torch.empty(max(int(L.dgb200_match_batch_workspace_bytes(off.ctypes.data_as(i32), len(counts),
+                                                                  pr.ctypes.data_as(i32), P)), 1),
+                     dtype=torch.uint8, device=dev)
+    x1 = x2 = None
+    kp_dim = out_dim = 0
+    if kbank is not None:
+        kp_dim = int(kbank.shape[1])
+        out_dim = 6 if kp_dim >= 6 else 2
+        x1 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
+        x2 = torch.empty((cap, out_dim), dtype=torch.float64, device=dev)
+    guided = ()
+    if guide is None:
+        fn = L.dgb200_match_binary_descriptors_batch_dev if hamming else L.dgb200_match_descriptors_batch_dev
+    else:
+        fn = (L.dgb200_match_binary_descriptors_guided_batch_dev if hamming else
+              L.dgb200_match_descriptors_guided_batch_dev)
+        guided = (models, int(guide), px_th)
+    _call(fn, L.dgb200_frontend_last_error, dev, bank, off.ctypes.data_as(i32), len(counts), D, pr.ctypes.data_as(i32),
+          P, *guided, ratio, int(bool(mutual)), kbank, kp_dim, mq, mt, x1, x2, out_dim, cap, offsets, ws)
     return BatchMatches(mq.long(), mt.long(), x1, x2, offsets, lay.n_max)
