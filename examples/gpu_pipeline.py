@@ -12,6 +12,9 @@
                                             ->  absolute pose by P3P RANSAC                (pydegensac_b200.matching)
                                             ->  3-view tracks triangulated across the registered views
                                             ->  views 1 and 2 and the tracks bundle-adjusted, view 0 held
+    and many views:                         ->  every pair matched and verified by the ragged F RANSAC
+                                            ->  tracks built from the verified matches   (pydegensac_b200.matching, CUDA)
+                                            ->  tracks triangulated with the views' poses
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -27,7 +30,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (find_absolute_pose_ragged, match_descriptors, match_descriptors_batch,
+from pydegensac_b200.matching import (build_tracks_ragged, find_absolute_pose_ragged, match_descriptors,
+                                      match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
                                       pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
                                       refine_pose_ragged, triangulate_tracks_ragged, bundle_adjust_ragged)
@@ -150,6 +154,38 @@ def register_third_view(dev, K):
           % (rot_err(R), rot_err(ba.R), float(np.median(err)), float(np.median(err_ba))))
 
 
+def tracks_across_views(dev, K, n_img=6):
+    """Every pair of n_img views matched and verified in one ragged batch, tracks built from the verified matches and
+    triangulated with the views' (planted) poses, without a host read until the report"""
+    kps, descs, poses, X, ids = synth_views(n_img=n_img, seed=5)
+    kt = [torch.from_numpy(k).to(dev) for k in kps]
+    dt = [torch.from_numpy(d).to(dev) for d in descs]
+    pairs = np.array([(i, j) for i in range(n_img) for j in range(i + 1, n_img)], dtype=np.int32)
+    m = match_descriptors_batch(dt, pairs, kt, ratio=0.9, mutual=True)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=list(range(len(pairs))),
+                                                    offsets=m.offsets, n_max=m.n_max)
+    ts = build_tracks_ragged([len(k) for k in kps], pairs, m.idx1, m.idx2, m.offsets, mask, kps=kt)
+    f64 = torch.float64
+    R = torch.from_numpy(np.stack([p[0] for p in poses])).to(dev, f64)
+    t = torch.from_numpy(np.stack([p[1] for p in poses])).to(dev, f64)
+    # the padded layout goes straight in: the empty tracks past the last one get no model
+    tr = triangulate_tracks_ragged(ts.cams, ts.pts, R, t, K, ts.offsets, px_th=2.0)
+    ex = trim_tracks(ts)                                      # the one host read of the track builder
+    off, cams, kp = ex.offsets.cpu().numpy(), ex.cams.cpu().numpy(), ex.kp.cpu().numpy()
+    T = len(off) - 1
+    pid = np.array([ids[c][k] for c, k in zip(cams, kp)])
+    pure = np.array([pid[off[j]] >= 0 and (pid[off[j]:off[j + 1]] == pid[off[j]]).all() for j in range(T)])
+    s = ts.stats.cpu().numpy()
+    print("%d views, %d pairs: %d tracks of %d observations (longest %d), %.1f %% of them pure; %d conflicting "
+          "components (%d keypoints) dropped" % (n_img, len(pairs), T, len(cams), int(np.diff(off).max()),
+                                                  100 * pure.mean(), int(s[2]), int(s[3])))
+    n_in = tr.n_inliers[:T].cpu().numpy()
+    ok = (n_in >= 2) & pure
+    err = np.linalg.norm(tr.X[:T].cpu().numpy()[ok] - X[pid[off[:-1]][ok]], axis=1)
+    print("  %d tracks triangulated with the planted poses, median 3D error %.2e units" % (int((n_in >= 2).sum()),
+                                                                                        float(np.median(err))))
+
+
 def main():
     dev = torch.device("cuda:0")
     kp1, d1, kp2, d2 = (torch.from_numpy(a).to(dev) for a in synth_features())
@@ -192,6 +228,7 @@ def main():
               " d = %.3f" % float(hp.plane[0, c, 3]))
     print("median parallax of the chosen pose: %.2f deg" % np.degrees(float(hp.median_angle[0])))
     register_third_view(dev, K)
+    tracks_across_views(dev, K)
 
 
 if __name__ == "__main__":

@@ -549,6 +549,44 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
                                     uint8_t* d_mask_out, double* d_cost0_out, double* d_cost_out,
                                     int32_t* d_iters_out, int32_t* d_n_used_out, void* stream);
 const char* dgb200_bundle_adjust_last_error(void);
+/* Tracks from verified pairwise matches (OpenMVG's TracksBuilder): the connected components of the graph whose nodes
+ * are the keypoints of all images and whose edges are the verified matches, in the ragged track layout that
+ * dgb200_triangulate_tracks_ragged_dev and dgb200_bundle_adjust_ragged_dev take.
+ *   Nodes: keypoint k of image i is node g = img_offsets[i] + k; img_offsets [n_images + 1] is a HOST prefix sum of the
+ *   images' keypoint counts (img_offsets[0] = 0, not decreasing), N = img_offsets[n_images] nodes.
+ *   Edges: pairs [n_pairs][2] is a HOST table of (query image q, train image t), as dgb200_match_descriptors_batch_dev
+ *   takes it, and pair p owns rows d_offsets[p] .. d_offsets[p+1]-1 of d_idx1 / d_idx2 (int32 [rows], keypoint
+ *   indices local to q and t) and d_mask (uint8 [rows] or NULL: every row), what the batch matcher and the ragged
+ *   RANSAC leave.  Pair p is well-formed when 0 <= d_offsets[p] <= d_offsets[p+1] <= rows; a pair that is not adds no
+ *   edge and none of its rows is read.  Row r of a well-formed pair is the edge (img_offsets[q] + d_idx1[r],
+ *   img_offsets[t] + d_idx2[r]) when d_mask[r] != 0 and both indices lie inside their images; any other row is
+ *   ignored.  Self-pairs (q = t) and repeated pairs or rows are allowed.
+ *   Tracks: the components of two or more nodes.  A component with two nodes of one image is conflicting and is
+ *   dropped whole (OpenMVG's rule); a component that survives with fewer than min_length nodes is dropped.
+ *   Order: tracks by their smallest node, the observations of a track by node, which is ascending image order.
+ * Outputs, capacity-sized because the number of tracks T is data-dependent (T_cap = N / min_length, rounded down):
+ * d_offsets_out int32 [T_cap + 1] (track j owns observations d_offsets_out[j] .. d_offsets_out[j+1]-1; the entries past
+ * T repeat the observation count, so they are empty tracks); d_cams_out int32 [N] the image (camera) of each
+ * observation and d_kp_out int32 [N] its keypoint index in that image; d_pts_out float64 [N][2] its pixel, copied from
+ * d_kp [N][2] (the keypoints' x, y in node order), when both are given; d_track_of_out int32 [N] the track of every
+ * node, or -1; d_stats_out int32 [4] = (tracks, observations, conflicting components, nodes in them).  Observation rows
+ * past the last track's are written as cams = kp = -1 and pts = NaN, so every byte of the output is specified.
+ * Determinism: the hooks of the union-find (csrc/tracks.h) leave each component's smallest node as its root whatever
+ * their order; the sizes and conflict counts are integer sums; the slot an atomic cursor gives a node in its track is
+ * undone by ranking the track's nodes.  So the output is a function of the edge set alone: permuting the pairs or the
+ * rows within a pair, or swapping a pair's direction together with idx1 / idx2, gives the same bytes.
+ * d_mask may be NULL; d_idx1 / d_idx2 may be NULL when rows = 0; d_cams_out, d_kp_out and d_track_of_out may be NULL
+ * when N = 0.  A null required buffer, n_images < 1, n_pairs < 1, rows < 0, min_length < 2, img_offsets that do not
+ * start at 0 or decrease, d_kp without d_pts_out (or the reverse), or a pair image index outside [0, n_images)
+ * returns DGB200_E_ARG before any launch; the message is dgb200_tracks_last_error()'s.  Asynchronous on `stream`:
+ * two copies of the host tables, 13 kernels and a stream-ordered workspace (cudaMallocAsync / cudaFreeAsync) of 22
+ * bytes per node, 16 per pair and 4 per image; nothing is read back. */
+int dgb200_build_tracks_ragged_dev(const int32_t* img_offsets, int n_images, const int32_t* pairs, int n_pairs,
+                                   const int32_t* d_idx1, const int32_t* d_idx2, const int32_t* d_offsets, int rows,
+                                   const uint8_t* d_mask, const double* d_kp, int min_length, int32_t* d_offsets_out,
+                                   int32_t* d_cams_out, int32_t* d_kp_out, double* d_pts_out, int32_t* d_track_of_out,
+                                   int32_t* d_stats_out, void* stream);
+const char* dgb200_tracks_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

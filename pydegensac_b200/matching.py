@@ -56,6 +56,11 @@ Tracks triangulated across the registered views (two-ray midpoint RANSAC with lo
 Cameras and points refined jointly (bundle adjustment, Levenberg-Marquardt with the Schur complement), view 0 held:
 
     ba = bundle_adjust_ragged(cams, pts, R, t, K, offsets, tr.X, mask=tr.mask, free=[1, 2], scale_gauge=1)
+
+The tracks themselves, built from the verified matches of many pairs (union-find over the keypoints of all images):
+
+    ts = build_tracks_ragged(counts, pairs, m.idx1, m.idx2, m.offsets, mask, kps=kps)
+    tr = triangulate_tracks_ragged(ts.cams, ts.pts, R, t, K, ts.offsets, px_th=2.0)
 """
 import collections
 import ctypes
@@ -76,6 +81,7 @@ RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost 
 AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
 Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
 BundleAdjustment = collections.namedtuple("BundleAdjustment", "R t X mask cost0 cost iters n_used")
+TrackSet = collections.namedtuple("TrackSet", "offsets cams kp pts track_of stats")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -88,11 +94,7 @@ def batch_layout(counts, pairs):
     query counts); col_prefix [P+1]: the pair's col_best segment (prefix of the train counts); capacity = row_prefix[P];
     n_max = the largest query-image count over the pairs (an upper bound on any pair's match count)."""
     c = np.asarray(counts, dtype=np.int64)
-    pr = np.asarray(pairs, dtype=np.int64)
-    if pr.ndim != 2 or pr.shape[1] != 2 or pr.shape[0] < 1:
-        raise ValueError("pairs must be a non-empty [P,2] array of (query image, train image)")
-    if pr.min() < 0 or pr.max() >= len(c):
-        raise ValueError("pairs: image index out of range")
+    pr = _check_pair_table(pairs, len(c))
     n1, n2 = c[pr[:, 0]], c[pr[:, 1]]
     tiles = np.where((n1 >= 1) & (n2 >= 2), (n1 + kTQ - 1) // kTQ, 0)
 
@@ -102,6 +104,16 @@ def batch_layout(counts, pairs):
         return out
     rows = prefix(n1)
     return BatchLayout(prefix(tiles), rows, prefix(n2), int(rows[-1]), int(n1.max()))
+
+
+def _check_pair_table(pairs, n_images):
+    """a host [P,2] table of (query image, train image) with P >= 1 and indices in [0, n_images); returns it as int64"""
+    pr = np.asarray(pairs, dtype=np.int64)
+    if pr.ndim != 2 or pr.shape[1] != 2 or pr.shape[0] < 1:
+        raise ValueError("pairs must be a non-empty [P,2] array of (query image, train image)")
+    if pr.min() < 0 or pr.max() >= n_images:
+        raise ValueError("pairs: image index out of range")
+    return pr
 
 
 def _check_norm(norm):
@@ -789,6 +801,97 @@ def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, s
           int(Kc.dim() == 3), C, off, T, obs, Xc, m, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr), gauge,
           sigma, max_iters, px_th, Ro, to, Xo, mo, cost0, cost, iters, n_used)
     return BundleAdjustment(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used)
+
+
+def build_tracks_ragged(counts, pairs, idx1, idx2, offsets, mask=None, kps=None, min_length=2):
+    """Build tracks from the verified matches of many image pairs: the connected components of the graph whose nodes
+    are the keypoints of all images and whose edges are the matches, in the ragged layout that
+    triangulate_tracks_ragged and bundle_adjust_ragged take (OpenMVG's TracksBuilder, on the device).
+
+    counts: a HOST sequence of the I images' keypoint counts (the node of keypoint k of image i is sum(counts[:i]) + k;
+    at most 2^31 - 1 nodes).  pairs: a HOST [P,2] table of (query image, train image), as match_descriptors_batch
+    takes it.  idx1, idx2 (int32 or int64 [rows]), offsets (int32 [P+1]) and mask ([rows] bool / uint8 or None: every
+    row) are CUDA tensors on one device: the BatchMatches fields and the ragged RANSAC mask, used as they are (int64
+    indices are narrowed on the device, out-of-range values staying out of range).  Row r of pair p = (q, t), with
+    offsets[p] <= r < offsets[p+1], joins keypoint idx1[r] of q and idx2[r] of t when the mask is set and both indices
+    lie inside their images; a pair whose offsets are not 0 <= offsets[p] <= offsets[p+1] <= rows adds nothing.
+    kps: optional list of I CUDA keypoint tensors [n_i, k >= 2]; their x, y (columns 0-1) become the observations'
+    pixels.  A component with two keypoints of one image is conflicting and dropped whole; a track needs at least
+    min_length (>= 2) keypoints.  Tracks are ordered by their smallest node, a track's observations by node (so by
+    image).  The estimator is specified in include/degensac_b200.h.
+    Returns TrackSet(offsets, cams, kp, pts, track_of, stats), capacity-sized because the number of tracks T is only
+    known on the device (N = sum(counts), T_cap = N // min_length): offsets int32 [T_cap+1] (entries past T repeat the
+    observation count: empty tracks, which triangulation and bundle adjustment leave alone); cams int32 [N] the image
+    of each observation; kp int32 [N] its keypoint index in that image; pts float64 [N,2] its pixel (None without kps);
+    track_of int32 [N] the track of each keypoint or -1; stats int32 [4] (tracks, observations, conflicting
+    components, keypoints in them).  Rows past the observations are cams = kp = -1, pts = NaN.  The output depends on
+    the set of matches alone, not on their order.  Asynchronous, nothing is read back; trim_tracks cuts it to size."""
+    import torch
+    if isinstance(counts, torch.Tensor) and counts.is_cuda:
+        raise ValueError("counts must be a host sequence: reading a CUDA tensor would synchronise")
+    pairs = _host_pairs(pairs)
+    cn = np.asarray(counts)
+    if cn.ndim != 1 or len(cn) < 1 or not np.issubdtype(cn.dtype, np.integer):
+        raise ValueError("counts must be a non-empty host sequence of integer keypoint counts")
+    cn = cn.astype(np.int64)
+    if cn.min() < 0:
+        raise ValueError("counts must not be negative")
+    if int(cn.sum()) > 2 ** 31 - 1:
+        raise ValueError("counts sum to %d keypoints, more than 2^31 - 1" % int(cn.sum()))
+    I = len(cn)
+    pr = np.ascontiguousarray(_check_pair_table(pairs, I), dtype=np.int32)
+    P = len(pr)
+    named = (("idx1", idx1), ("idx2", idx2), ("offsets", offsets))
+    _check_tensors(named, mask)
+    if idx1.dim() != 1:
+        raise ValueError("idx1 must be [rows], not %s" % list(idx1.shape))
+    rows = int(idx1.shape[0])
+    _check_shape("idx2", idx2, "rows", (rows,))
+    for nm, x in named[:2]:
+        if x.dtype not in (torch.int32, torch.int64):
+            raise ValueError("%s must be int32 or int64, not %s" % (nm, x.dtype))
+    _check_offsets(offsets, "P", P)
+    _check_mask(mask, "rows", rows)
+    min_length = _check_count("min_length", min_length, 2)
+    dev = _check_device(named, mask)
+    N = int(cn.sum())
+    kbank = None
+    if kps is not None:
+        if len(kps) != I or any(not isinstance(k, torch.Tensor) for k in kps):
+            raise ValueError("kps must hold one keypoint tensor per image (%d)" % I)
+        if any(k.dim() != 2 or k.shape[0] != c or k.shape[1] < 2 for k, c in zip(kps, cn)):
+            raise ValueError("keypoint tensors must be [n_i, k] with k >= 2 and n_i = counts[i]")
+        if any(k.device != dev for k in kps):
+            raise ValueError("kps must be on the device of idx1")
+        _check_floating([("kps", k) for k in kps])
+        kbank = torch.cat([k[:, :2].to(torch.float64) for k in kps], 0).contiguous() if N else None
+    i1, i2 = ((x if x.dtype == torch.int32 else x.clamp(-1, 2 ** 31 - 1).to(torch.int32)).contiguous()
+              for x in (idx1, idx2))
+    img_off = np.zeros(I + 1, dtype=np.int32)
+    img_off[1:] = np.cumsum(cn)
+    i32 = ctypes.POINTER(ctypes.c_int32)
+    L = _cabi.lib()
+    T_cap = N // min_length
+    off_out = torch.empty(T_cap + 1, dtype=torch.int32, device=dev)
+    cams = torch.empty(N, dtype=torch.int32, device=dev)
+    kp = torch.empty(N, dtype=torch.int32, device=dev)
+    pts = torch.empty((N, 2), dtype=torch.float64, device=dev) if kbank is not None else None
+    track_of = torch.empty(N, dtype=torch.int32, device=dev)
+    stats = torch.empty(4, dtype=torch.int32, device=dev)
+    _call(L.dgb200_build_tracks_ragged_dev, L.dgb200_tracks_last_error, dev, img_off.ctypes.data_as(i32), I,
+          pr.ctypes.data_as(i32), P, i1, i2, offsets.contiguous(), rows, _mask_u8(mask), kbank, min_length, off_out,
+          cams, kp, pts, track_of, stats)
+    if kps is not None and pts is None:
+        pts = torch.empty((0, 2), dtype=torch.float64, device=dev)
+    return TrackSet(off_out, cams, kp, pts, track_of, stats)
+
+
+def trim_tracks(ts):
+    """A TrackSet of build_tracks_ragged cut to its T tracks and their observations: one host read (of stats); the
+    tensors returned are views of the ones given."""
+    T, n = (int(v) for v in ts.stats[:2].tolist())
+    return TrackSet(ts.offsets[:T + 1], ts.cams[:n], ts.kp[:n], ts.pts[:n] if ts.pts is not None else None,
+                    ts.track_of, ts.stats)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
