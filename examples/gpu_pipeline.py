@@ -30,8 +30,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (build_tracks_ragged, find_absolute_pose_ragged, match_descriptors,
-                                      match_descriptors_batch, trim_tracks,
+from pydegensac_b200.matching import (build_tracks_ragged, bundle_adjust_pcg_ragged, find_absolute_pose_ragged,
+                                      match_descriptors, match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
                                       pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
                                       refine_pose_ragged, triangulate_tracks_ragged, bundle_adjust_ragged)
@@ -186,6 +186,51 @@ def tracks_across_views(dev, K, n_img=6):
                                                                                         float(np.median(err))))
 
 
+def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
+    """n_img views along a path, each matched with its next three and verified in one ragged batch, tracks built and
+    triangulated from perturbed planted poses, then one bundle adjustment of every view but view 0 -- more cameras
+    than bundle_adjust_ragged takes -- by conjugate gradients on the implicit Schur complement"""
+    rng = np.random.default_rng(seed)
+    X = np.c_[rng.uniform(-3, 0.3 * n_img + 3, n_pts), rng.uniform(-2, 2, n_pts), rng.uniform(4, 10, n_pts)]
+    code = rng.normal(size=(n_pts, D)).astype(np.float32)
+    Rs = np.stack([_rot("y", rng.uniform(-0.05, 0.05)) @ _rot("x", rng.uniform(-0.03, 0.03)) for _ in range(n_img)])
+    ts = -np.einsum("cij,cj->ci", Rs, np.c_[0.3 * np.arange(n_img), np.zeros((n_img, 2))])
+    kps, descs = [], []
+    for i in range(n_img):
+        q = (X @ Rs[i].T + ts[i]) @ _K.T
+        x = q[:, :2] / q[:, 2:3]
+        seen = np.flatnonzero((q[:, 2] > 0) & (x[:, 0] > 0) & (x[:, 0] < 640) & (x[:, 1] > 0) & (x[:, 1] < 480))
+        kps.append(torch.from_numpy(x[seen] + 0.3 * rng.normal(size=(len(seen), 2))).to(dev))
+        descs.append(torch.from_numpy(code[seen] + 0.15 * rng.normal(size=(len(seen), D)).astype(np.float32)).to(dev))
+    pairs = np.array([(i, j) for i in range(n_img) for j in range(i + 1, min(i + 4, n_img))], dtype=np.int32)
+    m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=list(range(len(pairs))),
+                                                    offsets=m.offsets, n_max=m.n_max)
+    tk = build_tracks_ragged([len(k) for k in kps], pairs, m.idx1, m.idx2, m.offsets, mask, kps=kps)
+    # the start: every view but view 0 rotated by ~2e-3 rad and moved by ~1e-2
+    R0, t0 = Rs.copy(), ts.copy()
+    for c in range(1, n_img):
+        a = 2e-3 * rng.normal(size=3)
+        A = np.array([[0.0, -a[2], a[1]], [a[2], 0.0, -a[0]], [-a[1], a[0], 0.0]])
+        th = np.linalg.norm(a)
+        R0[c] = (np.eye(3) + np.sin(th) / th * A + (1 - np.cos(th)) / th ** 2 * A @ A) @ Rs[c]
+        t0[c] = ts[c] + 1e-2 * rng.normal(size=3)
+    f64 = torch.float64
+    R, t = torch.from_numpy(R0).to(dev, f64), torch.from_numpy(t0).to(dev, f64)
+    tr = triangulate_tracks_ragged(tk.cams, tk.pts, R, t, K, tk.offsets, px_th=3.0)
+    gb = bundle_adjust_pcg_ragged(tk.cams, tk.pts, R, t, K, tk.offsets, tr.X, mask=tr.mask, loss_scale=1.0)
+
+    def rot_err(Rx):
+        Rx = Rx.cpu().numpy()
+        return np.degrees(max(np.arccos(np.clip((np.trace(Rx[c] @ Rs[c].T) - 1) / 2, -1, 1)) for c in range(n_img)))
+    n_tr = int(tk.stats[0])
+    print("%d views, %d pairs: %d tracks; global bundle adjustment of %d views over %d observations in %d trial steps "
+          "(%d CG iterations): cost %.1f -> %.1f" % (n_img, len(pairs), n_tr, n_img - 1, int(gb.n_used[0]),
+                                                      int(gb.iters[0]), int(gb.cg_iters[0]), float(gb.cost0[0]),
+                                                      float(gb.cost[0])))
+    print("  largest rotation error %.2e -> %.2e deg against the planted poses" % (rot_err(R), rot_err(gb.R)))
+
+
 def main():
     dev = torch.device("cuda:0")
     kp1, d1, kp2, d2 = (torch.from_numpy(a).to(dev) for a in synth_features())
@@ -229,6 +274,7 @@ def main():
     print("median parallax of the chosen pose: %.2f deg" % np.degrees(float(hp.median_angle[0])))
     register_third_view(dev, K)
     tracks_across_views(dev, K)
+    global_adjustment(dev, K)
 
 
 if __name__ == "__main__":

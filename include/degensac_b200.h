@@ -549,6 +549,43 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
                                     uint8_t* d_mask_out, double* d_cost0_out, double* d_cost_out,
                                     int32_t* d_iters_out, int32_t* d_n_used_out, void* stream);
 const char* dgb200_bundle_adjust_last_error(void);
+/* Bundle adjustment of any number of cameras (a global bundle adjustment of a whole reconstruction): the estimator of
+ * dgb200_bundle_adjust_ragged_dev with the reduced camera system solved inexactly by preconditioned conjugate
+ * gradients (PCG) on the Schur complement, which is never formed (Ceres' ITERATIVE_SCHUR with SCHUR_JACOBI).
+ * Everything is as there -- the track layout and conventions, the usable and used observations and the optimised
+ * tracks, the held and free cameras and scale_gauge with its device-chosen axis, the squared or Cauchy cost with IRLS
+ * weights, the parameterisation and the re-orthonormalisation of a trial R, the damping U* = U + lambda diag U and
+ * V* = V + lambda diag V, the back-substitution dX_p = -V*_p^-1 (g_p + sum_i W_i^T dc), the schedule, the output mask
+ * and the rule that held cameras and tracks that are not optimised are bit-identical to the input -- except:
+ *   Free cameras: h_free [n_free] is a HOST list of 0 to n_cams distinct camera indices, copied to the device.
+ *   Reduced system: S dc = b with S and b as the dense entry point defines them; the held coordinate and the cameras
+ *   without used observations are pinned to 0.  S p = U* p - sum_p W_p V*_p^-1 (W_p^T p) is computed matrix-free.
+ *   Preconditioner: block-diagonal, M_a = U*_a - sum_{i in a} W_i V*_p(i)^-1 W_i^T (6 x 6) per active free camera,
+ *   the held coordinate's row and column replaced by the identity's, each block Cholesky-factorised once per trial
+ *   step.  A non-positive pivot of M or of any V*_p rejects the step (lambda <- 10 lambda).
+ *   PCG: x0 = 0, r0 = b, z0 = M^-1 r0, p0 = z0, rho = r . z; b = 0 gives dc = 0.  Each iteration: q = S p, kappa =
+ *   p . q; kappa <= 0 or not finite stops (and rejects the step when it is the first iteration); alpha = rho / kappa,
+ *   x += alpha p, r -= alpha q; |r|_2 <= cg_tol |b|_2 or cg_max_iters iterations stop; else z = M^-1 r, rho' = r . z,
+ *   p = z + (rho' / rho) p, rho = rho'.  dc = x.
+ *   cg_max_iters >= 1, cg_tol >= 0 and finite.  d_cg_iters_out [1]: the products q = S p, summed over the trial steps.
+ * Every sum is reduced in a fixed order without atomics, the dot products of PCG included, over partitions that do not
+ * depend on the launch grid: a rerun gives the same bytes.  A null required buffer (d_cg_iters_out is one), n_free
+ * outside [0, n_cams], cg_max_iters < 1 or cg_tol not a non-negative finite number, and every case the dense entry
+ * point refuses, returns DGB200_E_ARG before any launch; the message is dgb200_bundle_adjust_pcg_last_error()'s.
+ * Asynchronous on `stream`: a copy of h_free, per trial step 6 launches whatever cg_max_iters is (the PCG loop is one
+ * cooperative launch sized by the occupancy API) and 10 around them, and a stream-ordered workspace (cudaMallocAsync /
+ * cudaFreeAsync) of 426 bytes per observation, 204 bytes per track, 468 bytes per camera, 760 bytes per free camera
+ * and 4 bytes per free camera and 4096 observations; nothing read back. */
+int dgb200_bundle_adjust_pcg_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R,
+                                        const double* d_t, const double* d_K, int k_per_camera, int n_cams,
+                                        const int32_t* d_offsets, int n_tracks, int obs, const double* d_X,
+                                        const uint8_t* d_mask, const int32_t* h_free, int n_free, int scale_gauge,
+                                        double loss_scale, int max_iters, double px_th, int cg_max_iters,
+                                        double cg_tol, double* d_R_out, double* d_t_out, double* d_X_out,
+                                        uint8_t* d_mask_out, double* d_cost0_out, double* d_cost_out,
+                                        int32_t* d_iters_out, int32_t* d_n_used_out, int32_t* d_cg_iters_out,
+                                        void* stream);
+const char* dgb200_bundle_adjust_pcg_last_error(void);
 /* Tracks from verified pairwise matches (OpenMVG's TracksBuilder): the connected components of the graph whose nodes
  * are the keypoints of all images and whose edges are the verified matches, in the ragged track layout that
  * dgb200_triangulate_tracks_ragged_dev and dgb200_bundle_adjust_ragged_dev take.

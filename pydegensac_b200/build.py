@@ -36,10 +36,12 @@ def build_cuda(force=False, verbose=False):
     src4 = os.path.join(CSRC, "triangulate.cu")    # multi-view triangulation of tracks across registered views
     src5 = os.path.join(CSRC, "bundle_adjust.cu")  # bundle adjustment of registered views and their tracks
     src6 = os.path.join(CSRC, "tracks.cu")         # tracks from verified pairwise matches (union-find over keypoints)
+    src7 = os.path.join(CSRC, "bundle_adjust_pcg.cu")  # bundle adjustment of any number of cameras (PCG on Schur)
     if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest(_csrc_files()):
         return LIB
     nvcc = os.environ.get("NVCC", "nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3, src4, src5, src6]
+    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3, src4, src5, src6,
+                                                                                 src7]
     subprocess.check_call(cmd)
     return LIB
 

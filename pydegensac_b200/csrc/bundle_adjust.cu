@@ -22,19 +22,23 @@
 //   ba_backsub_kernel   one warp per track: dX_p = -V*_p^-1 (g_p + sum W_i^T dc), the trial point and its cost;
 //   ba_decide_kernel    one CTA: fixed-order sum of the track costs, accept / reject / stop, lambda, buffer swap.
 // After the last step ba_finish_cameras_kernel and ba_finish_tracks_kernel write the outputs and the inlier mask.
-// No floating-point atomics anywhere: every sum has a fixed order, so a rerun gives the same bytes.
+// No floating-point atomics anywhere: every sum has a fixed order, so a rerun gives the same bytes.  The bodies of the
+// mark, init and finish kernels are in bundle_adjust_device.h and the argument checks in bundle_adjust_args.h, shared
+// with the iterative solver of bundle_adjust_pcg.cu.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 
 #include "../../include/degensac_b200.h"
 #include "entry_error.h"
+#include "bundle_adjust_args.h"
 #include "common.h"
 #include "absolute_pose.h"
 #include "pose_refine.h"
 #include "triangulate.h"
 #include "bundle_adjust.h"
 #include "device_util.h"
+#include "bundle_adjust_device.h"
 
 namespace {
 
@@ -44,14 +48,6 @@ int fail(int code, const char* what, cudaError_t e = cudaSuccess) { return set_e
 constexpr int kBaWarps = 4;                       // tracks (or Schur blocks) per CTA, one per warp
 constexpr int kBaThreads = 32 * kBaWarps;
 constexpr int kBaCamThreads = 128;
-constexpr int kBaCta = 1024;                      // the one-CTA kernels and the per-slot scans
-
-// The LM state of the call, in the workspace; only ba_init_kernel and ba_decide_kernel write it (bad: also the
-// kernels that find a non-positive pivot)
-struct BaState {
-  double lam, cost, cost0;
-  int cur, stop, lin, bad, iters, n_used, hold_row;
-};
 
 struct BaArgs {
   const int* cams; const double* pts;                      // [obs], [obs][2]
@@ -89,7 +85,6 @@ __device__ __forceinline__ const double* pose_of(const BaArgs& a, int buf, int c
 __device__ __forceinline__ double* point_of(const BaArgs& a, int buf, int j) {
   return a.Xb + 3 * ((size_t)buf * a.n_tracks + j);
 }
-__device__ __forceinline__ bool span_ok(const BaArgs& a, int b, int e) { return b >= 0 && b <= e && e <= a.obs; }
 __device__ __forceinline__ bool slot_active(const BaArgs& a, int s) { return a.list_off[s + 1] > a.list_off[s]; }
 
 __global__ void __launch_bounds__(kBaCamThreads) ba_cameras_kernel(BaArgs a) {
@@ -113,93 +108,7 @@ __global__ void __launch_bounds__(kBaThreads) ba_mark_kernel(BaArgs a) {
   const int lane = threadIdx.x & 31;
   const int j = blockIdx.x * kBaWarps + (threadIdx.x >> 5);
   if (j >= a.n_tracks) return;                       // (warp-uniform)
-  const double X[3] = {a.X[3 * (size_t)j], a.X[3 * (size_t)j + 1], a.X[3 * (size_t)j + 2]};
-  if (lane < 3) {
-    point_of(a, 0, j)[lane] = X[lane];
-    point_of(a, 1, j)[lane] = X[lane];
-  }
-  if (lane == 0) {
-    a.trk_used[j] = 0;
-    a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost] = 0.0;
-  }
-  const int b = a.offsets[j], e = a.offsets[j + 1];
-  if (!span_ok(a, b, e)) return;                     // malformed span: no row read or written
-  const bool xok = finite(X[0]) && finite(X[1]) && finite(X[2]);
-  // the usable observations; the camera of the first one and whether another camera sees the track too
-  int first_cam = -1, n = 0;
-  bool two = false;
-  double V[6] = {0, 0, 0, 0, 0, 0}, g[3] = {0, 0, 0}, cost = 0.0;
-  for (int c0 = b; c0 < e; c0 += 32) {
-    const int r = c0 + lane;
-    bool ok = false;
-    int cm = -1;
-    if (r < e) {
-      cm = a.cams[r];
-      const double x = a.pts[2 * (size_t)r], y = a.pts[2 * (size_t)r + 1];
-      ok = xok && (!a.mask || a.mask[r]) && cm >= 0 && cm < a.n_cams && finite(x) && finite(y) &&
-           a.tab[dg::kTrCamStride * (size_t)cm + dg::kTrCamOk] != 0.0;
-      if (ok) {
-        const double* P = pose_of(a, 0, cm);
-        const double* K = a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK;
-        double p[3];
-        dg::ap_camera(P, X[0], X[1], X[2], p);
-        ok = p[2] > 0.0;
-        if (ok) {
-          double rr[2], Jc[12], Jx[6];
-          dg::ba_jacobian(P, K, X, x, y, rr, Jc, Jx);
-          const double e2 = rr[0] * rr[0] + rr[1] * rr[1];
-          cost += dg::ba_rho(e2, a.sig2);
-          dg::ba_point_terms(Jx, rr, dg::ba_weight(e2, a.sig2), V, g);
-        }
-      }
-      a.usable[r] = ok ? 1 : 0;
-    }
-    const unsigned bal = __ballot_sync(kFull, ok);
-    if (bal) {
-      if (first_cam < 0) first_cam = __shfl_sync(kFull, cm, __ffs(bal) - 1);
-      two = two || __any_sync(kFull, ok && cm != first_cam);
-    }
-    n += __popc(bal);
-  }
-#pragma unroll
-  for (int s = 0; s < 6; ++s) V[s] = warp_sum(V[s]);
-  cost = warp_sum(cost);
-  double Vi[6];
-  const bool opt = two && dg::ba_inv3(V, 0.0, Vi);
-  __syncwarp();
-  for (int r = b + lane; r < e; r += 32) {
-    const unsigned char u = opt ? a.usable[r] : 0;
-    a.used[r] = u;
-    a.track_of[r] = j;
-  }
-  if (opt && lane == 0) {
-    a.trk_used[j] = n;
-    a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost] = cost;
-  }
-}
-
-__device__ int block_sum_int(int v, int* sh) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  v = warp_sum(v);
-  if (lane == 0) sh[wid] = v;
-  __syncthreads();
-  int total = 0;
-  for (int q = 0; q < kBaCta / 32; ++q) total += sh[q];
-  __syncthreads();
-  return total;
-}
-
-// A fixed-order sum over the CTA: thread i adds its terms in turn, then a tree over the threads
-__device__ double block_sum_double(double v, double* sh) {
-  sh[threadIdx.x] = v;
-  __syncthreads();
-  for (int s = kBaCta / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) sh[threadIdx.x] += sh[threadIdx.x + s];
-    __syncthreads();
-  }
-  const double total = sh[0];
-  __syncthreads();
-  return total;
+  ba_mark_track(a, j, lane);
 }
 
 __device__ __forceinline__ bool in_slot(const BaArgs& a, int r, int s) { return a.used[r] && a.slot_of[a.cams[r]] == s; }
@@ -239,37 +148,7 @@ __global__ void __launch_bounds__(kBaCta) ba_list_kernel(BaArgs a) {
   }
 }
 
-__global__ void __launch_bounds__(kBaCta) ba_init_kernel(BaArgs a) {
-  __shared__ double shd[kBaCta];
-  __shared__ int shi[kBaCta / 32];
-  double c = 0.0;
-  int u = 0;
-  for (int j = threadIdx.x; j < a.n_tracks; j += kBaCta) {
-    c += a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost];
-    u += a.trk_used[j];
-  }
-  c = block_sum_double(c, shd);
-  u = block_sum_int(u, shi);
-  if (threadIdx.x == 0) {
-    BaState* st = a.state;
-    st->lam = dg::kPrLambda0;
-    st->cost = c;
-    st->cost0 = c;
-    st->cur = 0;
-    st->stop = 0;
-    st->lin = 1;
-    st->bad = 0;
-    st->iters = 0;
-    st->n_used = u;
-    int hold = -1;
-    if (a.gauge_slot >= 0) {
-      const int ax = dg::ba_gauge_axis(pose_of(a, 0, a.free[a.gauge_slot]),
-                                       a.tab + dg::kTrCamStride * (size_t)a.held_cam + dg::kTrCamC);
-      hold = dg::kBaCamParams * a.gauge_slot + 3 + ax;
-    }
-    st->hold_row = hold;
-  }
-}
+__global__ void __launch_bounds__(kBaCta) ba_init_kernel(BaArgs a) { ba_init_state(a); }
 
 // ---------------------------------------------------------------------------------------------- one trial step
 __global__ void __launch_bounds__(kBaThreads) ba_linearise_kernel(BaArgs a) {
@@ -569,40 +448,14 @@ __global__ void __launch_bounds__(kBaCta) ba_decide_kernel(BaArgs a) {
 
 // ---------------------------------------------------------------------------------------------- outputs
 __global__ void __launch_bounds__(kBaCamThreads) ba_finish_cameras_kernel(BaArgs a) {
-  const BaState* st = a.state;
-  const int c = blockIdx.x * kBaCamThreads + threadIdx.x;
-  if (c == 0) {
-    a.cost0_out[0] = st->cost0;
-    a.cost_out[0] = st->cost;
-    a.iters_out[0] = st->iters;
-    a.n_used_out[0] = st->n_used;
-  }
-  if (c >= a.n_cams) return;
-  const double* P = pose_of(a, st->cur, c);
-  for (int i = 0; i < 9; ++i) a.R_out[9 * (size_t)c + i] = P[i];
-  for (int i = 0; i < 3; ++i) a.t_out[3 * (size_t)c + i] = P[9 + i];
+  ba_finish_camera(a, blockIdx.x * kBaCamThreads + threadIdx.x);
 }
 
 __global__ void __launch_bounds__(kBaThreads) ba_finish_tracks_kernel(BaArgs a) {
   const int lane = threadIdx.x & 31;
   const int j = blockIdx.x * kBaWarps + (threadIdx.x >> 5);
   if (j >= a.n_tracks) return;
-  const int cur = a.state->cur;
-  const double* X = point_of(a, cur, j);
-  if (lane < 3) a.X_out[3 * (size_t)j + lane] = X[lane];
-  const int b = a.offsets[j], e = a.offsets[j + 1];
-  if (!span_ok(a, b, e)) return;
-  for (int r = b + lane; r < e; r += 32) {
-    unsigned char f = 0;
-    if (a.usable[r]) {
-      const int cm = a.cams[r];
-      bool front;
-      const double e2 = dg::ap_sq_error(pose_of(a, cur, cm), a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK,
-                                        a.pts[2 * (size_t)r], a.pts[2 * (size_t)r + 1], X[0], X[1], X[2], &front);
-      f = front && e2 <= a.th2 ? 1 : 0;
-    }
-    a.mask_out[r] = f;
-  }
+  ba_finish_track(a, j, lane);
 }
 
 template <typename T>
@@ -625,33 +478,13 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
                                     int max_iters, double px_th, double* d_R_out, double* d_t_out, double* d_X_out,
                                     uint8_t* d_mask_out, double* d_cost0_out, double* d_cost_out,
                                     int32_t* d_iters_out, int32_t* d_n_used_out, void* stream) {
-  if (!d_R || !d_t || !d_K || !d_offsets || !d_X || !d_R_out || !d_t_out || !d_X_out || !d_cost0_out ||
-      !d_cost_out || !d_iters_out || !d_n_used_out)
-    return fail(DGB200_E_ARG, "null buffer");
-  if (obs > 0 && (!d_cams || !d_pts || !d_mask_out)) return fail(DGB200_E_ARG, "null observation buffer");
-  if (n_tracks < 1 || obs < 0 || n_cams < 1) return fail(DGB200_E_ARG, "need n_tracks >= 1, obs >= 0 and n_cams >= 1");
-  if (n_free < 0 || n_free > dg::kBaMaxFree) return fail(DGB200_E_ARG, "n_free must lie in [0, 64]");
-  if (n_free > 0 && !h_free) return fail(DGB200_E_ARG, "null free-camera list");
-  int gauge_slot = -1;
-  for (int q = 0; q < n_free; ++q) {
-    if (h_free[q] < 0 || h_free[q] >= n_cams) return fail(DGB200_E_ARG, "free camera index out of range");
-    for (int p = 0; p < q; ++p)
-      if (h_free[p] == h_free[q]) return fail(DGB200_E_ARG, "free camera index repeated");
-    if (h_free[q] == scale_gauge) gauge_slot = q;
-  }
-  if (scale_gauge >= 0 && gauge_slot < 0) return fail(DGB200_E_ARG, "scale_gauge must be one of the free cameras");
-  if (scale_gauge < -1) return fail(DGB200_E_ARG, "scale_gauge must be a free camera or -1");
-  int held_cam = -1;                                   // the lowest-index camera outside the free list
-  for (int c = 0; c < n_cams && held_cam < 0; ++c) {
-    bool is_free = false;
-    for (int q = 0; q < n_free; ++q) is_free = is_free || h_free[q] == c;
-    if (!is_free) held_cam = c;
-  }
-  if (gauge_slot >= 0 && held_cam < 0) return fail(DGB200_E_ARG, "scale_gauge needs a held camera");
-  if (!(loss_scale >= 0.0) || !(loss_scale < INFINITY))
-    return fail(DGB200_E_ARG, "loss_scale must be a positive number (or 0 for the trivial loss)");
-  if (max_iters < 0) return fail(DGB200_E_ARG, "max_iters must not be negative");
-  if (!(px_th > 0.0) || !(px_th < INFINITY)) return fail(DGB200_E_ARG, "px_th must be a positive number");
+  int gauge_slot = -1, held_cam = -1;
+  const char* bad = ba_arg_error(!d_R || !d_t || !d_K || !d_offsets || !d_X || !d_R_out || !d_t_out || !d_X_out ||
+                                     !d_cost0_out || !d_cost_out || !d_iters_out || !d_n_used_out,
+                                 !d_cams || !d_pts || !d_mask_out, n_tracks, obs, n_cams, h_free, n_free,
+                                 dg::kBaMaxFree, "n_free must lie in [0, 64]", scale_gauge, loss_scale, max_iters, px_th,
+                                 &gauge_slot, &held_cam);
+  if (bad) return fail(DGB200_E_ARG, bad);
   const cudaStream_t st = (cudaStream_t)stream;
   const int n = dg::kBaCamParams * n_free;
   const size_t no = (size_t)(obs > 0 ? obs : 1), nt = (size_t)n_tracks, nc = (size_t)n_cams;

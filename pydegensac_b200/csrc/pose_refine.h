@@ -174,6 +174,60 @@ DG_HD bool pr_cholesky_solve(const double* H, const double* g, double lam, doubl
 }
 DG_HD bool pr_solve(const double* H, const double* g, double lam, double* D) { return pr_cholesky_solve<5>(H, g, lam, D); }
 
+// The factor / apply pair of the same Cholesky, for one matrix and many right-hand sides (N = 6: the block-Jacobi
+// preconditioner of bundle_adjust_pcg.cu).  pr_cholesky_factor: A (upper triangle by rows [N (N + 1) / 2]) = L L^T,
+// L (lower triangle by rows, L[i][k] at i (i + 1) / 2 + k); false at a pivot that is not positive.
+// pr_cholesky_apply: x = A^-1 b from L (x may alias b).
+template <int N>
+DG_HD bool pr_cholesky_factor(const double* A, double* Lp) {
+  double L[N][N];
+  int m = 0;
+#pragma unroll
+  for (int k = 0; k < N; ++k)
+#pragma unroll
+    for (int l = k; l < N; ++l) L[l][k] = A[m++];
+#pragma unroll
+  for (int j = 0; j < N; ++j) {
+    double d = L[j][j];
+#pragma unroll
+    for (int k = 0; k < j; ++k) d -= L[j][k] * L[j][k];
+    if (!(d > 0.0)) return false;
+    L[j][j] = sqrt(d);
+#pragma unroll
+    for (int i = j + 1; i < N; ++i) {
+      double v = L[i][j];
+#pragma unroll
+      for (int k = 0; k < j; ++k) v -= L[i][k] * L[j][k];
+      L[i][j] = v / L[j][j];
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int k = 0; k <= i; ++k) Lp[i * (i + 1) / 2 + k] = L[i][k];
+  return true;
+}
+template <int N>
+DG_HD void pr_cholesky_apply(const double* Lp, const double* b, double* x) {
+  double y[N];
+#pragma unroll
+  for (int i = 0; i < N; ++i) {
+    double v = b[i];
+#pragma unroll
+    for (int k = 0; k < i; ++k) v -= Lp[i * (i + 1) / 2 + k] * y[k];
+    y[i] = v / Lp[i * (i + 1) / 2 + i];
+  }
+#pragma unroll
+  for (int i = N - 1; i >= 0; --i) {
+    double v = y[i];
+#pragma unroll
+    for (int k = i + 1; k < N; ++k) v -= Lp[k * (k + 1) / 2 + i] * y[k];
+    y[i] = v / Lp[i * (i + 1) / 2 + i];
+  }
+#pragma unroll
+  for (int i = 0; i < N; ++i) x[i] = y[i];
+}
+
 // The pose D = (w, d) away from (R, t): exp([w]x) = I + (sin a / a) [w]x + (2 sin^2(a/2) / a^2) [w]x^2, a = |w|
 DG_HD void pr_step(const double* R, const double* t, const double* D, double* R2, double* t2) {
   const double a = sqrt(D[0] * D[0] + D[1] * D[1] + D[2] * D[2]);

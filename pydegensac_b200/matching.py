@@ -81,6 +81,7 @@ RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost 
 AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
 Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
 BundleAdjustment = collections.namedtuple("BundleAdjustment", "R t X mask cost0 cost iters n_used")
+BundleAdjustmentPCG = collections.namedtuple("BundleAdjustmentPCG", "R t X mask cost0 cost iters n_used cg_iters")
 TrackSet = collections.namedtuple("TrackSet", "offsets cams kp pts track_of stats")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
@@ -717,6 +718,46 @@ def triangulate_tracks_ragged(cams, pts, R, t, K, offsets, mask=None, px_th=2.0,
 BA_MAX_FREE = 64   # free cameras per call at most (the reduced camera system is dense)
 
 
+def _check_ba_controls(free, scale_gauge, loss_scale, C, max_free=None):
+    """free, scale_gauge and loss_scale of the bundle adjustments over C cameras; max_free: the most free cameras
+    (None: no limit).  Returns (the free list, the gauge camera or -1, sigma or 0)"""
+    if free is None:
+        if max_free is not None and C - 1 > max_free:
+            raise ValueError("free=None frees %d cameras, more than %d: pass an explicit free list" % (C - 1, max_free))
+        free = list(range(1, C))
+    free = _host_pairs(free)
+    try:
+        fr = [int(c) for c in np.asarray(free).reshape(-1)]
+    except (TypeError, ValueError):
+        raise ValueError("free must be a host sequence of camera indices")
+    if max_free is not None and len(fr) > max_free:
+        raise ValueError("free holds %d cameras, more than %d" % (len(fr), max_free))
+    if len(set(fr)) != len(fr):
+        raise ValueError("free holds a camera twice")
+    if any(not 0 <= c < C for c in fr):
+        raise ValueError("free holds a camera index outside [0, %d)" % C)
+    n_held = C - len(fr)
+    if isinstance(scale_gauge, str):
+        if scale_gauge != "auto":
+            raise ValueError("scale_gauge must be 'auto', None or a camera of free, not %r" % (scale_gauge,))
+        gauge = fr[0] if n_held == 1 and fr else -1
+    elif scale_gauge is None:
+        gauge = -1
+    else:
+        gauge = int(scale_gauge)
+        if gauge not in fr:
+            raise ValueError("scale_gauge %d is not one of the free cameras" % gauge)
+        if n_held == 0:
+            raise ValueError("scale_gauge needs a held camera: every camera is free")
+    if loss_scale is None:
+        sigma = 0.0
+    else:
+        sigma = float(loss_scale)
+        if not 0.0 < sigma < float("inf"):
+            raise ValueError("loss_scale must be a positive number or None, not %r" % (loss_scale,))
+    return fr, gauge, sigma
+
+
 def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, scale_gauge="auto", loss_scale=None,
                          max_iters=50, px_th=2.0):
     """Bundle-adjust registered views and their tracks: Levenberg-Marquardt over the free cameras' poses and the
@@ -747,40 +788,7 @@ def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, s
     _check_shape("X", X, "T", (T, 3))
     _check_floating(named[1:5] + named[6:])
     _check_mask(mask, "obs", obs)
-    if free is None:
-        if C - 1 > BA_MAX_FREE:
-            raise ValueError("free=None frees %d cameras, more than %d: pass an explicit free list" % (C - 1, BA_MAX_FREE))
-        free = list(range(1, C))
-    free = _host_pairs(free)
-    try:
-        fr = [int(c) for c in np.asarray(free).reshape(-1)]
-    except (TypeError, ValueError):
-        raise ValueError("free must be a host sequence of camera indices")
-    if len(fr) > BA_MAX_FREE:
-        raise ValueError("free holds %d cameras, more than %d" % (len(fr), BA_MAX_FREE))
-    if len(set(fr)) != len(fr):
-        raise ValueError("free holds a camera twice")
-    if any(not 0 <= c < C for c in fr):
-        raise ValueError("free holds a camera index outside [0, %d)" % C)
-    n_held = C - len(fr)
-    if isinstance(scale_gauge, str):
-        if scale_gauge != "auto":
-            raise ValueError("scale_gauge must be 'auto', None or a camera of free, not %r" % (scale_gauge,))
-        gauge = fr[0] if n_held == 1 and fr else -1
-    elif scale_gauge is None:
-        gauge = -1
-    else:
-        gauge = int(scale_gauge)
-        if gauge not in fr:
-            raise ValueError("scale_gauge %d is not one of the free cameras" % gauge)
-        if n_held == 0:
-            raise ValueError("scale_gauge needs a held camera: every camera is free")
-    if loss_scale is None:
-        sigma = 0.0
-    else:
-        sigma = float(loss_scale)
-        if not 0.0 < sigma < float("inf"):
-            raise ValueError("loss_scale must be a positive number or None, not %r" % (loss_scale,))
+    fr, gauge, sigma = _check_ba_controls(free, scale_gauge, loss_scale, C, BA_MAX_FREE)
     max_iters = _check_count("max_iters", max_iters, 0)
     px_th = _check_px_th(px_th, True)
     dev = _check_device(named, mask)
@@ -801,6 +809,54 @@ def bundle_adjust_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, s
           int(Kc.dim() == 3), C, off, T, obs, Xc, m, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr), gauge,
           sigma, max_iters, px_th, Ro, to, Xo, mo, cost0, cost, iters, n_used)
     return BundleAdjustment(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used)
+
+
+def bundle_adjust_pcg_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=None, scale_gauge="auto", loss_scale=None,
+                             max_iters=50, px_th=2.0, cg_max_iters=100, cg_tol=0.1):
+    """Bundle-adjust any number of cameras: the Levenberg-Marquardt of bundle_adjust_ragged, with the reduced camera
+    system solved inexactly by conjugate gradients on the implicit Schur complement and a block-Jacobi preconditioner
+    (Ceres' ITERATIVE_SCHUR with SCHUR_JACOBI), so that it has no camera limit.  It is a different estimator from
+    bundle_adjust_ragged: each trial step is the exact LM step only up to the CG tolerance.
+
+    The arguments are bundle_adjust_ragged's, except: free is a HOST sequence of any number of distinct camera
+    indices (None: every camera but camera 0, whatever their number); cg_max_iters >= 1 bounds the CG iterations of
+    each trial step, and cg_tol >= 0 stops them once |r| <= cg_tol |b| (0.1, the default, is Ceres' inexact-Newton
+    forcing value).  The estimator is specified in include/degensac_b200.h.
+    Returns BundleAdjustmentPCG(R, t, X, mask, cost0, cost, iters, n_used, cg_iters): bundle_adjust_ragged's fields and
+    cg_iters [1] int32, the CG iterations summed over the trial steps.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("K", K), ("offsets", offsets), ("X", X))
+    _check_tensors(named, mask)
+    T, obs, C = _check_tracks(cams, pts, R, t, K, offsets)
+    _check_shape("X", X, "T", (T, 3))
+    _check_floating(named[1:5] + named[6:])
+    _check_mask(mask, "obs", obs)
+    fr, gauge, sigma = _check_ba_controls(free, scale_gauge, loss_scale, C)
+    max_iters = _check_count("max_iters", max_iters, 0)
+    px_th = _check_px_th(px_th, True)
+    cg_max_iters = _check_count("cg_max_iters", cg_max_iters, 1)
+    cg_tol = float(cg_tol)
+    if not 0.0 <= cg_tol < float("inf"):
+        raise ValueError("cg_tol must be a non-negative finite number, not %r" % (cg_tol,))
+    dev = _check_device(named, mask)
+    x, Rc, tc, Kc, Xc = _f64(pts, R, t, K, X)
+    cm, off, m = cams.contiguous(), offsets.contiguous(), _mask_u8(mask)
+    hf = np.ascontiguousarray(fr, dtype=np.int32)
+    f64 = torch.float64
+    L = _cabi.lib()
+    Ro = torch.empty((C, 3, 3), dtype=f64, device=dev)
+    to = torch.empty((C, 3), dtype=f64, device=dev)
+    Xo = torch.empty((T, 3), dtype=f64, device=dev)
+    mo = _rows_out(obs, dev)
+    cost0 = torch.empty(1, dtype=f64, device=dev)
+    cost = torch.empty(1, dtype=f64, device=dev)
+    iters = torch.empty(1, dtype=torch.int32, device=dev)
+    n_used = torch.empty(1, dtype=torch.int32, device=dev)
+    cg_iters = torch.empty(1, dtype=torch.int32, device=dev)
+    _call(L.dgb200_bundle_adjust_pcg_ragged_dev, L.dgb200_bundle_adjust_pcg_last_error, dev, cm, x, Rc, tc, Kc,
+          int(Kc.dim() == 3), C, off, T, obs, Xc, m, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr), gauge,
+          sigma, max_iters, px_th, cg_max_iters, cg_tol, Ro, to, Xo, mo, cost0, cost, iters, n_used, cg_iters)
+    return BundleAdjustmentPCG(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used, cg_iters)
 
 
 def build_tracks_ragged(counts, pairs, idx1, idx2, offsets, mask=None, kps=None, min_length=2):
