@@ -30,7 +30,8 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (build_tracks_ragged, bundle_adjust_pcg_ragged, find_absolute_pose_ragged,
+from pydegensac_b200.matching import (build_tracks_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
+                                      find_absolute_pose_ragged, undistort_points,
                                       match_descriptors, match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
                                       pose_from_homography_ragged, refine_fundamental_ragged, refine_homography_ragged,
@@ -231,6 +232,57 @@ def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
     print("  largest rotation error %.2e -> %.2e deg against the planted poses" % (rot_err(R), rot_err(gb.R)))
 
 
+
+def self_calibration(dev, n_img=20, n_pts=4000, seed=9):
+    """Views through a lens with radial distortion (f = 520, k1 = -0.08, k2 = 0.01), known tracks, and a start with a
+    focal length 5 % off and no distortion: undistort, triangulate, adjust poses, points and the intrinsics of the one
+    camera, then undistort again with the refined intrinsics and re-triangulate"""
+    rng = np.random.default_rng(seed)
+    k_true = np.array([520.0, 320.0, 240.0, -0.08, 0.01])
+    X = np.c_[rng.uniform(-3, 0.3 * n_img + 3, n_pts), rng.uniform(-2, 2, n_pts), rng.uniform(4, 10, n_pts)]
+    Rs = np.stack([_rot("y", rng.uniform(-0.05, 0.05)) @ _rot("x", rng.uniform(-0.03, 0.03)) for _ in range(n_img)])
+    ts = -np.einsum("cij,cj->ci", Rs, np.c_[0.3 * np.arange(n_img), np.zeros((n_img, 2))])
+    cams, pts, off = [], [], [0]
+    for j in range(n_pts):
+        p = np.einsum("cij,j->ci", Rs, X[j]) + ts
+        u = p[:, :2] / p[:, 2:]
+        s = (u ** 2).sum(1)
+        x = (k_true[0] * (1 + s * (k_true[3] + s * k_true[4])))[:, None] * u + k_true[1:3]
+        seen = np.flatnonzero((x[:, 0] > 0) & (x[:, 0] < 640) & (x[:, 1] > 0) & (x[:, 1] < 480))
+        cams.append(seen)
+        pts.append(x[seen] + 0.3 * rng.normal(size=(len(seen), 2)))
+        off.append(off[-1] + len(seen))
+    f64, i32 = torch.float64, torch.int32
+    cams = torch.from_numpy(np.concatenate(cams).astype(np.int32)).to(dev)
+    pts = torch.from_numpy(np.concatenate(pts)).to(dev)
+    off = torch.tensor(off, dtype=i32, device=dev)
+    R, t = torch.from_numpy(Rs).to(dev, f64), torch.from_numpy(ts).to(dev, f64)
+    groups = torch.zeros(n_img, dtype=i32, device=dev)                 # one camera for every view
+    k0 = k_true.copy()
+    k0[0] *= 1.05
+    k0[3:] = 0.0
+    intr = torch.from_numpy(k0[None]).to(dev)
+
+    def pinhole(k):
+        return torch.tensor([[k[0], 0.0, k[1]], [0.0, k[0], k[2]], [0.0, 0.0, 1.0]], dtype=f64, device=dev)
+
+    def triangulate(k):
+        und = undistort_points(pts, cams, groups, torch.from_numpy(k[None]).to(dev))
+        return triangulate_tracks_ragged(cams, und, R, t, pinhole(k), off, px_th=4.0)
+
+    tr = triangulate(k0)
+    sc = bundle_adjust_intrinsics_ragged(cams, pts, R, t, groups, intr, off, tr.X, mask=tr.mask, loss_scale=1.0)
+    k1 = sc.intrinsics[0].cpu().numpy()
+    tr2 = triangulate(k1)
+
+    def med_err(Xe):
+        return float(np.nanmedian(np.linalg.norm(Xe.cpu().numpy() - X, axis=1)))
+    print("self-calibration of %d views over %d observations in %d trial steps (%d CG iterations): cost %.1f -> %.1f"
+          % (n_img, int(sc.n_used[0]), int(sc.iters[0]), int(sc.cg_iters[0]), float(sc.cost0[0]), float(sc.cost[0])))
+    print("  focal error %.2f -> %.3f px, k1 error %.2e -> %.2e; median 3D error %.2e -> %.2e units after "
+          "re-triangulation" % (abs(k0[0] - k_true[0]), abs(k1[0] - k_true[0]), abs(k0[3] - k_true[3]),
+                                abs(k1[3] - k_true[3]), med_err(tr.X), med_err(tr2.X)))
+
 def main():
     dev = torch.device("cuda:0")
     kp1, d1, kp2, d2 = (torch.from_numpy(a).to(dev) for a in synth_features())
@@ -275,6 +327,7 @@ def main():
     register_third_view(dev, K)
     tracks_across_views(dev, K)
     global_adjustment(dev, K)
+    self_calibration(dev)
 
 
 if __name__ == "__main__":

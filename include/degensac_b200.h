@@ -586,6 +586,72 @@ int dgb200_bundle_adjust_pcg_ragged_dev(const int32_t* d_cams, const double* d_p
                                         int32_t* d_iters_out, int32_t* d_n_used_out, int32_t* d_cg_iters_out,
                                         void* stream);
 const char* dgb200_bundle_adjust_pcg_last_error(void);
+/* Bundle adjustment with intrinsics: the estimator of dgb200_bundle_adjust_pcg_ragged_dev over the free cameras' poses,
+ * the free intrinsics groups' parameters and the tracks' points jointly, with the RADIAL camera model (COLMAP's):
+ *   camera c of group g = d_groups[c], intrinsics k_g = d_intrinsics[g] = (f, cx, cy, k1, k2) float64 [n_groups][5]:
+ *   p = R_c X + t_c, u = (p0 / p2, p1 / p2), s = u . u, pixel = f (1 + k1 s + k2 s^2) u + (cx, cy).
+ *   One focal length (no fx != fy), no skew, no tangential terms.  With k1 = k2 = 0 this is the pinhole projection of
+ *   the other entry points with K = [[f, 0, cx], [0, f, cy], [0, 0, 1]].
+ * Everything is as in dgb200_bundle_adjust_pcg_ragged_dev (usable and used observations, optimised tracks, scale gauge,
+ * loss, IRLS weights, LM schedule, PCG stopping rules, outputs, determinism, pass-through), except:
+ *   Cameras: a camera whose group index lies outside [0, n_groups), or whose group's parameters are not all finite or
+ *   have f <= 0, is treated as an unregistered camera: its observations are not usable.
+ *   Free groups: h_free_groups [n_free_groups] is a HOST list of 0 to n_groups distinct group indices, copied to the
+ *   device.  refine is a set of DGB200_REFINE_* bits: the coordinates of each free group that move, f (FOCAL), (cx, cy)
+ *   (PRINCIPAL_POINT), (k1, k2) (DISTORTION); with refine = 0 no group is free.  The others are pinned.  A free group
+ *   without a used observation is pinned whole and passed through.  Observations of held cameras constrain their
+ *   group's intrinsics; their poses do not move.
+ *   Reduced system: over [free poses (6 each); free groups' intrinsics (5 each)], pinned coordinates with identity rows
+ *   and columns and a zero right-hand side.  With J_pose, J_intr, J_X the observations' Jacobians and w their IRLS
+ *   weights, U = sum w J^T J over [pose; intrinsics] is not block-diagonal: camera a of group g adds the cross block
+ *   E_a = sum_{i in a} w J_pose,i^T J_intr,i.  W_i = w [J_pose,i; J_intr,i]^T J_X,i.  U* = U + lambda diag U over every
+ *   kept coordinate, the intrinsics included.  S p = U* p - sum_p W_p V*_p^-1 W_p^T p, matrix-free: per PCG iteration
+ *   y_p = V*_p^-1 sum_i (W_pose,i^T p_cam(i) + W_intr,i^T p_grp(i)), q_a = U*_aa p_a + E_a p_g(a) - sum_{i in a}
+ *   W_pose,i y, q_g = U*_gg p_g + sum_{a in g} E_a^T p_a - sum_{i in g} W_intr,i y.
+ *   Preconditioner (Ceres' SCHUR_JACOBI): block-diagonal over the parameter blocks, the 6 x 6 pose block of the PCG
+ *   entry point per free camera and M_g = U*_gg - sum_{i in g} W_intr,i V*^-1 W_intr,i^T (5 x 5, pinned rows and
+ *   columns of the identity) per free group; the cross blocks are left out.
+ *   Trial step: intrinsics k_g + dk_g for the active free groups; a trial f <= 0 costs +inf, so the step is rejected.
+ *   Sums over a group, which may own every observation, are taken over a fixed partition of the group-major list of
+ *   its used observations (a stable counting sort) into chunks of 256, each chunk's partial sum in a fixed tree over a
+ *   warp and the chunks summed in order: no floating-point atomics, the same bytes for any grid.
+ * Outputs: bundle_adjust_pcg's, and d_intrinsics_out [n_groups][5] (held groups and inactive free groups bit-identical
+ * to the input); the mask is taken at the refined intrinsics.  Outputs may alias the inputs (R, t, X, intrinsics).
+ * A null required buffer (d_groups, d_intrinsics and d_intrinsics_out are), n_groups < 1, n_free_groups outside
+ * [0, n_groups], a null h_free_groups with n_free_groups > 0, a free group index out of range or repeated, refine with
+ * a bit outside DGB200_REFINE_*, and every case dgb200_bundle_adjust_pcg_ragged_dev refuses, returns DGB200_E_ARG
+ * before any launch (the shared checks first, in that entry point's order); the message is
+ * dgb200_bundle_adjust_intrinsics_last_error()'s.  Asynchronous on `stream`: copies of h_free and h_free_groups, per
+ * trial step at most 8 launches whatever cg_max_iters is (the PCG loop is one cooperative launch sized by the occupancy
+ * API) and at most 27 copies, memsets and launches around them, and a stream-ordered workspace (cudaMallocAsync /
+ * cudaFreeAsync) of 962 bytes per observation plus 356 per 256 observations, 204 bytes per track, 468 per camera, 84
+ * per group, 760 per free camera, 920 per free group, and 4 per 4096 observations times the larger of the free camera
+ * and free group counts; nothing is read back. */
+#define DGB200_REFINE_FOCAL 1
+#define DGB200_REFINE_PRINCIPAL_POINT 2
+#define DGB200_REFINE_DISTORTION 4
+int dgb200_bundle_adjust_intrinsics_ragged_dev(
+    const int32_t* d_cams, const double* d_pts, const double* d_R, const double* d_t, const int32_t* d_groups,
+    const double* d_intrinsics, int n_groups, int n_cams, const int32_t* d_offsets, int n_tracks, int obs,
+    const double* d_X, const uint8_t* d_mask, const int32_t* h_free, int n_free, const int32_t* h_free_groups,
+    int n_free_groups, int refine, int scale_gauge, double loss_scale, int max_iters, double px_th, int cg_max_iters,
+    double cg_tol, double* d_R_out, double* d_t_out, double* d_X_out, double* d_intrinsics_out, uint8_t* d_mask_out,
+    double* d_cost0_out, double* d_cost_out, int32_t* d_iters_out, int32_t* d_n_used_out, int32_t* d_cg_iters_out,
+    void* stream);
+const char* dgb200_bundle_adjust_intrinsics_last_error(void);
+/* Undistortion through the RADIAL model: d_out [rows][2] float64 = the pinhole pixel f u + (cx, cy) of each raw pixel
+ * d_pts [rows][2] of camera d_cams[r] (int32) in group d_groups[c] (int32 [n_cams]), intrinsics d_intrinsics
+ * [n_groups][5] as above.  The pinhole pixels feed the entry points that take K = [[f, 0, cx], [0, f, cy], [0, 0, 1]].
+ * One thread per row: the undistorted radius rho solves rho (1 + k1 rho^2 + k2 rho^4) = |pixel - c| / f by Newton's
+ * method bracketed in [0, the first turning point of the distortion] (a step that leaves the bracket bisects it), at
+ * most 50 steps, converged at a relative step of 1e-15.  NaN for a row whose camera or group index is out of range,
+ * whose group's intrinsics are not finite or have f <= 0, whose pixel is not finite, whose radius lies at or beyond
+ * the image of the turning point, or that does not converge.  A null d_groups or d_intrinsics, a null row buffer with
+ * rows > 0, rows < 0, n_cams < 1 or n_groups < 1 returns DGB200_E_ARG (message: dgb200_undistort_last_error());
+ * asynchronous on `stream`, one launch, no workspace. */
+int dgb200_undistort_points_dev(const double* d_pts, const int32_t* d_cams, int rows, const int32_t* d_groups,
+                                int n_cams, const double* d_intrinsics, int n_groups, double* d_out, void* stream);
+const char* dgb200_undistort_last_error(void);
 /* Tracks from verified pairwise matches (OpenMVG's TracksBuilder): the connected components of the graph whose nodes
  * are the keypoints of all images and whose edges are the verified matches, in the ragged track layout that
  * dgb200_triangulate_tracks_ragged_dev and dgb200_bundle_adjust_ragged_dev take.

@@ -86,6 +86,12 @@ def lib():
         L.dgb200_bundle_adjust_pcg_ragged_dev.argtypes = [vp, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, vp, i32, ci, ci, cd,
                                                           ci, cd, ci, cd, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
         L.dgb200_bundle_adjust_pcg_last_error.restype = ctypes.c_char_p
+        L.dgb200_bundle_adjust_intrinsics_ragged_dev.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, vp, i32,
+                                                                 ci, i32, ci, ci, ci, cd, ci, cd, ci, cd, vp, vp, vp,
+                                                                 vp, vp, vp, vp, vp, vp, vp, vp]
+        L.dgb200_bundle_adjust_intrinsics_last_error.restype = ctypes.c_char_p
+        L.dgb200_undistort_points_dev.argtypes = [vp, vp, ci, vp, ci, vp, ci, vp, vp]
+        L.dgb200_undistort_last_error.restype = ctypes.c_char_p
         L.dgb200_build_tracks_ragged_dev.argtypes = [i32, ci, i32, ci, vp, vp, vp, ci, vp, vp, ci, vp, vp, vp, vp, vp, vp,
                                                      vp]
         L.dgb200_tracks_last_error.restype = ctypes.c_char_p

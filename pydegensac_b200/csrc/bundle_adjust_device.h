@@ -1,12 +1,15 @@
 // bundle_adjust_device.h -- the kernel bodies that the dense bundle adjustment (bundle_adjust.cu) and the iterative one
-// (bundle_adjust_pcg.cu) share: the LM state, the fixed-order CTA sums, the marking of the usable observations and
-// optimised tracks, the start state, the step decision (bundle_adjust_pcg.cu only) and the outputs.  Device code, in the anonymous namespace of the
+// (bundle_adjust_pcg.cu) share, with the one that also refines the intrinsics (bundle_adjust_intrinsics.cu): the LM
+// state, the fixed-order CTA sums, the counting sort of the observations (bundle_adjust_intrinsics.cu only), the marking
+// of the usable observations and optimised tracks, the start state, the step decision (not bundle_adjust.cu) and the
+// outputs.  Device code, in the anonymous namespace of the
 // including translation unit (after device_util.h), as each kernel source keeps its own.
 //
 // The templates take the translation unit's argument block A, which has the members used here with the meaning they
 // have in bundle_adjust.cu's BaArgs: the inputs (cams, pts, mask, offsets, X, n_cams, n_tracks, obs, sig2, th2), the
 // free list (free, gauge_slot, held_cam), the workspace (tab, poses [2][n_cams][12], Xb [2][T][3], trk, usable, used,
-// track_of, trk_used, state) and the outputs.
+// track_of, trk_used, state) and the outputs.  The marking and the output mask also take the camera model Cam: BaPinhole,
+// the camera table's K, unless the caller passes its own (bundle_adjust_intrinsics.cu: the RADIAL model).
 #pragma once
 #include <cuda_runtime.h>
 
@@ -23,6 +26,21 @@ constexpr int kBaCta = 1024;                      // the one-CTA kernels
 struct BaState {
   double lam, cost, cost0;
   int cur, stop, lin, bad, iters, n_used, hold_row;
+};
+
+// The pinhole model of the camera table: an observation's residual r [2] and J_X [2][3] under pose P, and its e^2
+struct BaPinhole {
+  template <class A>
+  static __device__ __forceinline__ void point_row(const A& a, const double* P, int cm, int /*buf*/, const double* X,
+                                                   double x, double y, double* r, double* Jx) {
+    double Jc[12];
+    dg::ba_jacobian(P, a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK, X, x, y, r, Jc, Jx);
+  }
+  template <class A>
+  static __device__ __forceinline__ double sq_error(const A& a, const double* P, int cm, int /*buf*/, const double* X,
+                                                    double x, double y, bool* front) {
+    return dg::ap_sq_error(P, a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK, x, y, X[0], X[1], X[2], front);
+  }
 };
 
 __device__ int block_sum_int(int v, int* sh) {
@@ -49,8 +67,74 @@ __device__ double block_sum_double(double v, double* sh) {
   return total;
 }
 
+// The one-digit stable counting sort of the observations by a key in [0, n_keys) (-1: left out), in three passes.
+// Warp w owns observations [w range, (w + 1) range) and column w of hist [n_keys][n_ranges], so its updates need no
+// atomics.  ba_sort_count: the counts; ba_sort_scan (one CTA of kBaCta threads, sh: kBaCta ints): their exclusive
+// prefix sum in key-major order, in place, and list_off [n_keys + 1] the start of each key; ba_sort_scatter: pos_of
+// [obs] the position of each observation in the key-major list, ascending observation order within a key, and item
+// [position] = track_of of its observation.  bundle_adjust_pcg.cu keeps these bodies written out in its pcg_hist,
+// pcg_scan and pcg_scatter kernels: calling them there changes those kernels' register allocation and instructions.
+__device__ __forceinline__ void ba_sort_count(const int* key, int obs, int range, int* hist, int n_ranges, int w,
+                                              int lane) {
+  const int r0 = w * range, r1 = min(r0 + range, obs);
+  for (int c0 = r0; c0 < r1; c0 += 32) {
+    const int r = c0 + lane;
+    const int s = r < r1 ? key[r] : -1;
+    const unsigned peers = __match_any_sync(kFull, s);
+    if (s >= 0 && lane == __ffs(peers) - 1) hist[(size_t)s * n_ranges + w] += __popc(peers);
+    __syncwarp();
+  }
+}
+
+__device__ __forceinline__ void ba_sort_scan(int* hist, int n_keys, int n_ranges, int* list_off, int* sh) {
+  const size_t n = (size_t)n_keys * n_ranges;
+  const size_t per = (n + kBaCta - 1) / kBaCta;
+  const size_t b = per * threadIdx.x, e = min(b + per, n);
+  int sum = 0;
+  for (size_t i = b; i < e; ++i) sum += hist[i];
+  sh[threadIdx.x] = sum;
+  __syncthreads();
+  if (threadIdx.x == 0) {                            // 1024 partial sums, scanned in order by one thread
+    int run = 0;
+    for (int q = 0; q < kBaCta; ++q) {
+      const int v = sh[q];
+      sh[q] = run;
+      run += v;
+    }
+    list_off[n_keys] = run;
+  }
+  __syncthreads();
+  int run = sh[threadIdx.x];
+  for (size_t i = b; i < e; ++i) {
+    const int v = hist[i];
+    hist[i] = run;
+    if (i % n_ranges == 0) list_off[i / n_ranges] = run;
+    run += v;
+  }
+}
+
+__device__ __forceinline__ void ba_sort_scatter(const int* key, int obs, int range, int* hist, int n_ranges,
+                                                const int* track_of, int* pos_of, int* item, int w, int lane) {
+  const int r0 = w * range, r1 = min(r0 + range, obs);
+  for (int c0 = r0; c0 < r1; c0 += 32) {
+    const int r = c0 + lane;
+    const int s = r < r1 ? key[r] : -1;
+    const unsigned peers = __match_any_sync(kFull, s);
+    if (s >= 0) {
+      int* cursor = hist + (size_t)s * n_ranges + w;
+      const int base = *cursor;
+      const int pos = base + __popc(peers & ((1u << lane) - 1u));
+      pos_of[r] = pos;
+      item[pos] = track_of[r];
+      __syncwarp(peers);                               // every peer has read the cursor before the first one moves it
+      if (lane == __ffs(peers) - 1) *cursor = base + __popc(peers);
+    }
+    __syncwarp();
+  }
+}
+
 // One warp per track j: the usable observations, whether the track is optimised, its start cost, both point buffers
-template <class A>
+template <class A, class Cam = BaPinhole>
 __device__ __forceinline__ void ba_mark_track(const A& a, int j, int lane) {
   const double X[3] = {a.X[3 * (size_t)j], a.X[3 * (size_t)j + 1], a.X[3 * (size_t)j + 2]};
   if (lane < 3) {
@@ -79,13 +163,12 @@ __device__ __forceinline__ void ba_mark_track(const A& a, int j, int lane) {
            a.tab[dg::kTrCamStride * (size_t)cm + dg::kTrCamOk] != 0.0;
       if (ok) {
         const double* P = a.poses + 12 * (size_t)cm;
-        const double* K = a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK;
         double p[3];
         dg::ap_camera(P, X[0], X[1], X[2], p);
         ok = p[2] > 0.0;
         if (ok) {
-          double rr[2], Jc[12], Jx[6];
-          dg::ba_jacobian(P, K, X, x, y, rr, Jc, Jx);
+          double rr[2], Jx[6];
+          Cam::point_row(a, P, cm, 0, X, x, y, rr, Jx);
           const double e2 = rr[0] * rr[0] + rr[1] * rr[1];
           cost += dg::ba_rho(e2, a.sig2);
           dg::ba_point_terms(Jx, rr, dg::ba_weight(e2, a.sig2), V, g);
@@ -199,7 +282,7 @@ __device__ __forceinline__ void ba_finish_camera(const A& a, int c) {
 }
 
 // One warp per track j: the output point and the track's rows of the output mask
-template <class A>
+template <class A, class Cam = BaPinhole>
 __device__ __forceinline__ void ba_finish_track(const A& a, int j, int lane) {
   const int cur = a.state->cur;
   const double* X = a.Xb + 3 * ((size_t)cur * a.n_tracks + j);
@@ -211,9 +294,8 @@ __device__ __forceinline__ void ba_finish_track(const A& a, int j, int lane) {
     if (a.usable[r]) {
       const int cm = a.cams[r];
       bool front;
-      const double e2 = dg::ap_sq_error(a.poses + 12 * ((size_t)cur * a.n_cams + cm),
-                                        a.tab + dg::kTrCamStride * (size_t)cm + dg::kTrCamK, a.pts[2 * (size_t)r],
-                                        a.pts[2 * (size_t)r + 1], X[0], X[1], X[2], &front);
+      const double e2 = Cam::sq_error(a, a.poses + 12 * ((size_t)cur * a.n_cams + cm), cm, cur, X,
+                                      a.pts[2 * (size_t)r], a.pts[2 * (size_t)r + 1], &front);
       f = front && e2 <= a.th2 ? 1 : 0;
     }
     a.mask_out[r] = f;

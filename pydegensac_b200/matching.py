@@ -82,6 +82,8 @@ AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters 
 Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
 BundleAdjustment = collections.namedtuple("BundleAdjustment", "R t X mask cost0 cost iters n_used")
 BundleAdjustmentPCG = collections.namedtuple("BundleAdjustmentPCG", "R t X mask cost0 cost iters n_used cg_iters")
+BundleAdjustmentIntrinsics = collections.namedtuple("BundleAdjustmentIntrinsics",
+                                                    "R t X intrinsics mask cost0 cost iters n_used cg_iters")
 TrackSet = collections.namedtuple("TrackSet", "offsets cams kp pts track_of stats")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
@@ -857,6 +859,126 @@ def bundle_adjust_pcg_ragged(cams, pts, R, t, K, offsets, X, mask=None, free=Non
           int(Kc.dim() == 3), C, off, T, obs, Xc, m, hf.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), len(fr), gauge,
           sigma, max_iters, px_th, cg_max_iters, cg_tol, Ro, to, Xo, mo, cost0, cost, iters, n_used, cg_iters)
     return BundleAdjustmentPCG(Ro, to, Xo, mo.view(torch.bool), cost0, cost, iters, n_used, cg_iters)
+
+
+def _check_groups(groups, intrinsics, C):
+    """groups int32 [C] and intrinsics [G,5] of the RADIAL model; returns G"""
+    _check_int32("groups", groups)
+    _check_shape("groups", groups, "C", (C,))
+    if intrinsics.dim() != 2 or intrinsics.shape[0] < 1 or intrinsics.shape[1] != 5:
+        raise ValueError("intrinsics must be [G,5] with G >= 1, not %s" % list(intrinsics.shape))
+    return int(intrinsics.shape[0])
+
+
+def bundle_adjust_intrinsics_ragged(cams, pts, R, t, groups, intrinsics, offsets, X, mask=None, free=None,
+                                    free_groups=None, refine_focal=True, refine_principal_point=False,
+                                    refine_distortion=True, scale_gauge="auto", loss_scale=None, max_iters=50,
+                                    px_th=2.0, cg_max_iters=100, cg_tol=0.1):
+    """Bundle adjustment that also refines the intrinsics: the estimator of bundle_adjust_pcg_ragged over the free
+    cameras' poses, the free intrinsics groups and the tracks' points, with COLMAP's RADIAL camera model.
+
+    The camera model: p = R X + t, u = p[:2] / p[2], s = u . u, pixel = f (1 + k1 s + k2 s^2) u + (cx, cy), with the
+    intrinsics (f, cx, cy, k1, k2) of the camera's group.  One focal length and no skew, by design; with k1 = k2 = 0 it
+    is the pinhole K = [[f, 0, cx], [0, f, cy], [0, 0, 1]] of the other entry points.
+    groups: int32 [C] CUDA tensor, the row of intrinsics [G,5] (a floating CUDA tensor) that each camera uses: one group
+    for every view of one camera, arange(C) for a camera per view.  A camera whose group index lies outside [0, G), or
+    whose group's parameters are not finite or have f <= 0, is treated as an unregistered camera.
+    free_groups: a HOST sequence of distinct group indices whose intrinsics move (None: every group).  refine_focal,
+    refine_principal_point, refine_distortion: which of f, (cx, cy) and (k1, k2) move in a free group (COLMAP's
+    defaults).  A free group without a used observation is passed through.  Observations of held cameras constrain
+    their group's intrinsics.  The other arguments are bundle_adjust_pcg_ragged's.  The estimator is specified in
+    include/degensac_b200.h.
+    Returns BundleAdjustmentIntrinsics(R, t, X, intrinsics, mask, cost0, cost, iters, n_used, cg_iters):
+    bundle_adjust_pcg_ragged's fields and intrinsics [G,5] float64 (held groups bit-identical to the input); the mask is
+    taken at the refined intrinsics.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("cams", cams), ("pts", pts), ("R", R), ("t", t), ("groups", groups), ("intrinsics", intrinsics),
+             ("offsets", offsets), ("X", X))
+    _check_tensors(named, mask)
+    T = _check_offsets(offsets, "T")
+    _check_int32("cams", cams)
+    obs = _check_columns("pts", pts, "obs", 2)
+    _check_shape("cams", cams, "obs", (obs,))
+    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
+        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
+    C = int(R.shape[0])
+    _check_shape("t", t, "C", (C, 3))
+    G = _check_groups(groups, intrinsics, C)
+    _check_shape("X", X, "T", (T, 3))
+    _check_floating((("pts", pts), ("R", R), ("t", t), ("intrinsics", intrinsics), ("X", X)))
+    _check_mask(mask, "obs", obs)
+    fr, gauge, sigma = _check_ba_controls(free, scale_gauge, loss_scale, C)
+    if free_groups is None:
+        fg = list(range(G))
+    else:
+        try:
+            fg = [int(g) for g in np.asarray(_host_pairs(free_groups)).reshape(-1)]
+        except (TypeError, ValueError):
+            raise ValueError("free_groups must be a host sequence of group indices")
+        if len(set(fg)) != len(fg):
+            raise ValueError("free_groups holds a group twice")
+        if any(not 0 <= g < G for g in fg):
+            raise ValueError("free_groups holds a group index outside [0, %d)" % G)
+    refine = (1 if refine_focal else 0) | (2 if refine_principal_point else 0) | (4 if refine_distortion else 0)
+    max_iters = _check_count("max_iters", max_iters, 0)
+    px_th = _check_px_th(px_th, True)
+    cg_max_iters = _check_count("cg_max_iters", cg_max_iters, 1)
+    cg_tol = float(cg_tol)
+    if not 0.0 <= cg_tol < float("inf"):
+        raise ValueError("cg_tol must be a non-negative finite number, not %r" % (cg_tol,))
+    dev = _check_device(named, mask)
+    x, Rc, tc, kc, Xc = _f64(pts, R, t, intrinsics, X)
+    cm, gr, off, m = cams.contiguous(), groups.contiguous(), offsets.contiguous(), _mask_u8(mask)
+    hf = np.ascontiguousarray(fr, dtype=np.int32)
+    hg = np.ascontiguousarray(fg, dtype=np.int32)
+    f64 = torch.float64
+    L = _cabi.lib()
+    Ro = torch.empty((C, 3, 3), dtype=f64, device=dev)
+    to = torch.empty((C, 3), dtype=f64, device=dev)
+    Xo = torch.empty((T, 3), dtype=f64, device=dev)
+    ko = torch.empty((G, 5), dtype=f64, device=dev)
+    mo = _rows_out(obs, dev)
+    cost0 = torch.empty(1, dtype=f64, device=dev)
+    cost = torch.empty(1, dtype=f64, device=dev)
+    iters = torch.empty(1, dtype=torch.int32, device=dev)
+    n_used = torch.empty(1, dtype=torch.int32, device=dev)
+    cg_iters = torch.empty(1, dtype=torch.int32, device=dev)
+    i32p = ctypes.POINTER(ctypes.c_int32)
+    _call(L.dgb200_bundle_adjust_intrinsics_ragged_dev, L.dgb200_bundle_adjust_intrinsics_last_error, dev, cm, x, Rc,
+          tc, gr, kc, G, C, off, T, obs, Xc, m, hf.ctypes.data_as(i32p), len(fr), hg.ctypes.data_as(i32p), len(fg),
+          refine, gauge, sigma, max_iters, px_th, cg_max_iters, cg_tol, Ro, to, Xo, ko, mo, cost0, cost, iters, n_used,
+          cg_iters)
+    return BundleAdjustmentIntrinsics(Ro, to, Xo, ko, mo.view(torch.bool), cost0, cost, iters, n_used, cg_iters)
+
+
+def undistort_points(pts, cams, groups, intrinsics):
+    """The pinhole pixels of raw pixels through the RADIAL model of bundle_adjust_intrinsics_ragged.
+
+    pts [obs,2] floating, cams int32 [obs] the camera of each row, groups int32 [C] and intrinsics [G,5] (f, cx, cy, k1,
+    k2): CUDA tensors on one device.  Returns float64 [obs,2], f u + (cx, cy) for the undistorted normalised point u of
+    each row, which triangulate_tracks_ragged and find_absolute_pose_ragged take with K = [[f, 0, cx], [0, f, cy],
+    [0, 0, 1]] of the row's group.  A row whose camera or group index is out of range, whose group's intrinsics are not
+    finite or have f <= 0, whose radius lies beyond the first turning point of the distortion, or whose Newton
+    iteration does not converge, gives NaN.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("pts", pts), ("cams", cams), ("groups", groups), ("intrinsics", intrinsics))
+    _check_tensors(named, None)
+    obs = _check_columns("pts", pts, "obs", 2)
+    _check_int32("cams", cams)
+    _check_shape("cams", cams, "obs", (obs,))
+    _check_int32("groups", groups)
+    if groups.dim() != 1 or groups.shape[0] < 1:
+        raise ValueError("groups must be [C] with C >= 1, not %s" % list(groups.shape))
+    C = int(groups.shape[0])
+    G = _check_groups(groups, intrinsics, C)
+    _check_floating((("pts", pts), ("intrinsics", intrinsics)))
+    dev = _check_device(named, None)
+    x, kc = _f64(pts, intrinsics)
+    out = torch.empty((obs, 2), dtype=torch.float64, device=dev)
+    L = _cabi.lib()
+    _call(L.dgb200_undistort_points_dev, L.dgb200_undistort_last_error, dev, x, cams.contiguous(), obs,
+          groups.contiguous(), C, kc, G, out)
+    return out
 
 
 def build_tracks_ragged(counts, pairs, idx1, idx2, offsets, mask=None, kps=None, min_length=2):
