@@ -15,6 +15,7 @@
     and many views:                         ->  every pair matched and verified by the ragged F RANSAC
                                             ->  tracks built from the verified matches   (pydegensac_b200.matching, CUDA)
                                             ->  tracks triangulated with the views' poses
+                                            ->  every view's rotation averaged over the view graph (CUDA)
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -30,7 +31,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (build_tracks_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
+from pydegensac_b200.matching import (average_rotations, build_tracks_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
                                       find_absolute_pose_ragged, undistort_points,
                                       match_descriptors, match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
@@ -187,10 +188,9 @@ def tracks_across_views(dev, K, n_img=6):
                                                                                         float(np.median(err))))
 
 
-def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
-    """n_img views along a path, each matched with its next three and verified in one ragged batch, tracks built and
-    triangulated from perturbed planted poses, then one bundle adjustment of every view but view 0 -- more cameras
-    than bundle_adjust_ragged takes -- by conjugate gradients on the implicit Schur complement"""
+def path_scene(dev, n_img=100, n_pts=20000, D=64, seed=7):
+    """n_img views along a path looking at one scene, with keypoints and descriptors on the device, and the pairs of
+    each view with its next three.  Returns (rng, planted rotations, planted translations, kps, descs, pairs)"""
     rng = np.random.default_rng(seed)
     X = np.c_[rng.uniform(-3, 0.3 * n_img + 3, n_pts), rng.uniform(-2, 2, n_pts), rng.uniform(4, 10, n_pts)]
     code = rng.normal(size=(n_pts, D)).astype(np.float32)
@@ -204,6 +204,14 @@ def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
         kps.append(torch.from_numpy(x[seen] + 0.3 * rng.normal(size=(len(seen), 2))).to(dev))
         descs.append(torch.from_numpy(code[seen] + 0.15 * rng.normal(size=(len(seen), D)).astype(np.float32)).to(dev))
     pairs = np.array([(i, j) for i in range(n_img) for j in range(i + 1, min(i + 4, n_img))], dtype=np.int32)
+    return rng, Rs, ts, kps, descs, pairs
+
+
+def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
+    """n_img views along a path, each matched with its next three and verified in one ragged batch, tracks built and
+    triangulated from perturbed planted poses, then one bundle adjustment of every view but view 0 -- more cameras
+    than bundle_adjust_ragged takes -- by conjugate gradients on the implicit Schur complement"""
+    rng, Rs, ts, kps, descs, pairs = path_scene(dev, n_img, n_pts, D, seed)
     m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
     F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=list(range(len(pairs))),
                                                     offsets=m.offsets, n_max=m.n_max)
@@ -230,6 +238,66 @@ def global_adjustment(dev, K, n_img=100, n_pts=20000, D=64, seed=7):
                                                       int(gb.iters[0]), int(gb.cg_iters[0]), float(gb.cost0[0]),
                                                       float(gb.cost[0])))
     print("  largest rotation error %.2e -> %.2e deg against the planted poses" % (rot_err(R), rot_err(gb.R)))
+
+
+def view_graph_scene(dev, n_bad=6, seed=11):
+    """The path scene of global_adjustment and n_bad long-range pairs (i, i + 40) whose relative rotation will be a
+    random one (a wrong pose that passed verification); the random rotations are uploaded here, before the device
+    pipeline runs"""
+    scene = path_scene(dev)
+    n_img = len(scene[1])
+    rng = np.random.default_rng(seed)
+    first = rng.choice(n_img - 40, n_bad, replace=False)
+    bad = np.c_[first, first + 40].astype(np.int32)
+    q, _ = np.linalg.qr(rng.normal(size=(n_bad, 3, 3)))
+    q *= np.sign(np.linalg.det(q))[:, None, None]
+    return scene + (bad, torch.from_numpy(q).to(dev))
+
+
+def view_graph_rotations(dev, K, scene):
+    """Every pair of the scene matched, verified by the ragged F RANSAC, posed and refined; the bad pairs appended with
+    their random rotations and a support of 30; then the rotations averaged over the view graph, ranked by the pairs'
+    support -- the spanning-tree start alone, and the whole estimator.  No host read."""
+    _, Rs, _, kps, descs, pairs, bad, R_bad = scene
+    m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
+    seeds = torch.arange(len(pairs), dtype=torch.int64, device=dev)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=seeds, offsets=m.offsets,
+                                                    n_max=m.n_max)
+    pose = pose_from_fundamental_ragged(F, K, K, m.pts1, m.pts2, m.offsets, mask)
+    fine = refine_pose_ragged(pose.R, pose.t, K, K, m.pts1, m.pts2, m.offsets, pose.in_front, px_th=1.0)
+    all_pairs = np.r_[pairs, bad]
+    R_rel = torch.cat([fine.R, R_bad])
+    good = torch.cat([pose.good, torch.full((len(bad),), 30, dtype=torch.int32, device=dev)])
+    start = average_rotations(all_pairs, R_rel, len(Rs), weights=good, l1_iters=0, max_iters=0)
+    return start, average_rotations(all_pairs, R_rel, len(Rs), weights=good)
+
+
+def report_view_graph(scene, out):
+    """Prints the largest rotation error of the start and of the result against the planted rotations (the gauge
+    aligned at view 0), in degrees, and returns them"""
+    Rs, pairs, bad = scene[1], scene[5], scene[6]
+    start, ra = out
+
+    def largest(R):
+        R = R.cpu().numpy()
+        R = R @ (R[0].T @ Rs[0])
+        return np.degrees(max(np.arccos(np.clip((np.trace(R[c] @ Rs[c].T) - 1) / 2, -1, 1)) for c in range(len(Rs))))
+    e0, e1 = largest(start.R), largest(ra.R)
+    res = np.degrees(ra.residual.cpu().numpy())
+    print("rotation averaging of %d views over %d verified pairs and %d wrong ones: %s L1 and %s Geman-McClure "
+          "iterations (%d CG); residual of the wrong pairs %.1f deg at least, of the others %.3f deg at most"
+          % (len(Rs), len(pairs), len(bad), *ra.iters.cpu().tolist(), int(ra.cg_iters[0]), res[len(pairs):].min(),
+             np.nanmax(res[:len(pairs)])))
+    print("  largest rotation error %.3f deg from the spanning tree, %.3f deg averaged (against the planted rotations)"
+          % (e0, e1))
+    return e0, e1
+
+
+def rotations_from_view_graph(dev, K):
+    """A world rotation for each of 100 views from the verified relative poses of their pairs, a few wrong pairs
+    among them"""
+    scene = view_graph_scene(dev)
+    report_view_graph(scene, view_graph_rotations(dev, K, scene))
 
 
 
@@ -327,6 +395,7 @@ def main():
     register_third_view(dev, K)
     tracks_across_views(dev, K)
     global_adjustment(dev, K)
+    rotations_from_view_graph(dev, K)
     self_calibration(dev)
 
 

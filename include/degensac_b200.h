@@ -690,6 +690,54 @@ int dgb200_build_tracks_ragged_dev(const int32_t* img_offsets, int n_images, con
                                    int32_t* d_cams_out, int32_t* d_kp_out, double* d_pts_out, int32_t* d_track_of_out,
                                    int32_t* d_stats_out, void* stream);
 const char* dgb200_tracks_last_error(void);
+/* Rotation averaging over a view graph (the first step of global SfM, as GLOMAP's rotation averager): a world rotation
+ * for every view from the relative rotations of its verified pairs.  Translations are neither used nor produced.
+ *   Edges: h_pairs [n_pairs][2] is a HOST table of (i, j), as dgb200_match_descriptors_batch_dev takes it; d_R_rel
+ *   float64 [n_pairs][9] row-major with x_j ~ R_e x_i, so R_e ~ R_j R_i^T (what dgb200_pose_from_fundamental_ragged_dev
+ *   returns for the pair (q, t) = (i, j)); d_mask uint8 [n_pairs] or NULL (every edge); d_weights int32 [n_pairs] or
+ *   NULL (all 0): each edge's priority in the spanning tree, such as the pose's count of points in front.
+ *   1 Valid edge: i != j, the mask set, weight >= 0, R_e finite with det R_e > 0.5 (a failed pose's R = 0 drops out).
+ *     A valid R_e whose largest |R R^T - I| entry exceeds 1e-12 is re-orthonormalised (Gram-Schmidt on the rows).
+ *   2 Components: the connected components of the valid edges, each rooted at its smallest view.  A view without a
+ *     valid edge gets R = NaN and component -1.
+ *   3 Start: the maximum spanning forest under the strict order "e before f iff w_e > w_f, or w_e = w_f and e < f"
+ *     (unique; Boruvka rounds on the key ((INT32_MAX - w) << 32) | e).  Each root gets R = I; along each tree edge the
+ *     child's rotation is its parent's composed with the edge's, R_j = R_e R_i or R_i = R_e^T R_j.
+ *   4 Residual of a valid edge: dR_e = R_j^T R_e R_i, r_e = log dR_e, theta_e = |r_e| in [0, pi]: with a = (dR32 -
+ *     dR23, dR13 - dR31, dR21 - dR12), theta = atan2(|a|, tr dR - 1), r = theta / (2 sin theta) a, by its Taylor
+ *     series below theta = 1e-4; within 1e-3 of pi the axis is the largest-diagonal column of (dR + dR^T) / 2 - cos
+ *     theta I, normalised and signed as a.  Finite for every rotation.
+ *   5 Linearisation: right perturbations R_v <- R_v exp([w_v]x) (w in the world frame) change r_e by -w_j + w_i to
+ *     first order, so each iteration solves min sum_e w_e |w_j - w_i - r_e|^2 with w = 0 at every root: the weighted
+ *     graph Laplacian (x) I_3 with each root's row and column replaced by the identity's and its right-hand side 0.
+ *     The update R_v <- exp([R_v w_v]x) R_v is re-orthonormalised when it drifts more than 1e-12.
+ *   6 Weights: phase 1 (L1, Weiszfeld) w_e = 1 / max(theta_e, 1e-3) for at most l1_iters iterations, then phase 2
+ *     (Geman-McClure, rho = sigma^2 theta^2 / (sigma^2 + theta^2)) w_e = (sigma^2 / (sigma^2 + theta_e^2))^2 for at
+ *     most max_iters.  A phase ends early once max_v |w_v| <= step_tol after that iteration's update.  With l1_iters =
+ *     max_iters = 0 the output is the start.
+ *   7 Solve: Jacobi-preconditioned CG over the 3 n_views unknowns (diagonal sum_{e in v} w_e, 1 on roots), with the
+ *     stopping rules of dgb200_bundle_adjust_pcg_ragged_dev: x0 = 0; |r| <= cg_tol |b| or cg_max_iters iterations
+ *     stop; kappa = p . q <= 0 or not finite stops, and on the first iteration the iteration makes no update and ends
+ *     its phase.  S p is matrix-free over a view-major list of the valid edges (ascending edge order within a view).
+ * Outputs: d_R_out float64 [n_views][9] world-to-camera (x ~ K (R X + t), the convention of
+ * dgb200_find_absolute_pose_ragged_dev, triangulation and bundle adjustment); d_component_out int32 [n_views];
+ * d_residual_out float64 [n_pairs] theta_e at the output (NaN for an edge that is not valid); d_iters_out int32 [2]
+ * the iterations of each phase; d_cg_iters_out int32 [1] the products S p, summed over the iterations.
+ * Determinism: no floating-point atomics; the dot products and per-view sums are taken over partitions that do not
+ * depend on the launch grid, so a rerun gives the same bytes.  A null required buffer (d_mask and d_weights are not),
+ * n_views < 1, n_pairs < 1, a null h_pairs, a view index outside [0, n_views), sigma not a positive finite number,
+ * negative l1_iters or max_iters, step_tol or cg_tol not a non-negative finite number, or cg_max_iters < 1 returns
+ * DGB200_E_ARG before any launch; the message is dgb200_rotation_averaging_last_error()'s.  Asynchronous on `stream`:
+ * a copy of h_pairs, 5 launches, 3 per Boruvka round, one cooperative launch for the start, 4 per iteration whatever
+ * cg_max_iters is (the CG loop is one cooperative launch sized by the occupancy API; every kernel returns at once once
+ * the call has stopped) and 2 for the outputs, and a stream-ordered workspace (cudaMallocAsync / cudaFreeAsync) of 146
+ * bytes per edge, 308 bytes per view and 4 bytes per view and 2048 edges; nothing is read back. */
+int dgb200_average_rotations_dev(const int32_t* h_pairs, int n_pairs, int n_views, const double* d_R_rel,
+                                 const uint8_t* d_mask, const int32_t* d_weights, double sigma, int l1_iters,
+                                 int max_iters, double step_tol, int cg_max_iters, double cg_tol, double* d_R_out,
+                                 int32_t* d_component_out, double* d_residual_out, int32_t* d_iters_out,
+                                 int32_t* d_cg_iters_out, void* stream);
+const char* dgb200_rotation_averaging_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);
