@@ -16,6 +16,8 @@
                                             ->  tracks built from the verified matches   (pydegensac_b200.matching, CUDA)
                                             ->  tracks triangulated with the views' poses
                                             ->  every view's rotation averaged over the view graph (CUDA)
+                                            ->  every view's position and every track's point from the rotations
+                                            ->  tracks triangulated on the positioning's inliers, bundle-adjusted
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -31,7 +33,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (average_rotations, build_tracks_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
+from pydegensac_b200.matching import (average_rotations, build_tracks_ragged, global_positioning_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
                                       find_absolute_pose_ragged, undistort_points,
                                       match_descriptors, match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
@@ -301,6 +303,69 @@ def rotations_from_view_graph(dev, K):
 
 
 
+def global_reconstruction_run(dev, K, scene):
+    """Global SfM on the path scene with no pose from outside and no host read: every pair matched, verified by the
+    ragged F RANSAC, posed and refined; the rotations averaged over the view graph; tracks built from the verified
+    matches (their padded layout as it is); the views' positions and the tracks' points from the rotations; the tracks
+    triangulated on the positioning's inliers; one bundle adjustment of every view but view 0.  Returns (rotation
+    averaging, positioning, triangulation, bundle adjustment)"""
+    _, Rs, _, kps, descs, pairs = scene
+    m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
+    seeds = torch.arange(len(pairs), dtype=torch.int64, device=dev)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=seeds, offsets=m.offsets,
+                                                    n_max=m.n_max)
+    pose = pose_from_fundamental_ragged(F, K, K, m.pts1, m.pts2, m.offsets, mask)
+    fine = refine_pose_ragged(pose.R, pose.t, K, K, m.pts1, m.pts2, m.offsets, pose.in_front, px_th=1.0)
+    ra = average_rotations(pairs, fine.R, len(Rs), weights=pose.good)
+    tk = build_tracks_ragged([len(k) for k in kps], pairs, m.idx1, m.idx2, m.offsets, mask, kps=kps)
+    gpos = global_positioning_ragged(tk.cams, tk.pts, ra.R, K, tk.offsets)
+    tr = triangulate_tracks_ragged(tk.cams, tk.pts, ra.R, gpos.t, K, tk.offsets, mask=gpos.inliers, px_th=3.0)
+    ba = bundle_adjust_pcg_ragged(tk.cams, tk.pts, ra.R, gpos.t, K, tk.offsets, tr.X, mask=tr.mask, loss_scale=1.0)
+    return ra, gpos, tr, ba
+
+
+def similarity_errors(R, t, Rs, ts):
+    """The errors against the planted poses after the similarity world_true = s Q world_est + tau that best fits them:
+    Q from the rotations (the chordal mean, R_true ~ R_est Q^T: the path's centres lie on a line, so they leave the
+    rotation about it open), then s and tau from the centres by least squares.  Returns (centre errors in units of the
+    planted scene, rotation errors in degrees)"""
+    M = np.einsum("cji,cjk->ik", R, Rs)               # sum R_est^T R_true
+    U, _, Vt = np.linalg.svd(M)
+    G = U @ np.diag([1.0, 1.0, np.sign(np.linalg.det(U @ Vt))]) @ Vt
+    Ra = R @ G                                         # G = Q^T
+    er = np.degrees(np.arccos(np.clip((np.einsum("cij,cij->c", Ra, Rs) - 1.0) / 2.0, -1.0, 1.0)))
+    C = -np.einsum("cji,cj->ci", R, t)
+    Ct = -np.einsum("cji,cj->ci", Rs, ts)
+    A = (C - C.mean(0)) @ G                            # Q (C - mean), row by row
+    B = Ct - Ct.mean(0)
+    s = np.sum(A * B) / np.sum(A * A)
+    ec = np.linalg.norm(s * A - B, axis=1)
+    return ec, er
+
+
+def report_global_reconstruction(scene, out):
+    """Prints the centre and rotation errors against the planted poses after positioning and after bundle adjustment,
+    and returns the largest of each: (centre after positioning, centre after BA, rotation after BA in degrees)"""
+    _, Rs, ts = scene[:3]
+    ra, gpos, tr, ba = out
+    R = ra.R.cpu().numpy()
+    c0, r0 = similarity_errors(R, gpos.t.cpu().numpy(), Rs, ts)
+    c1, r1 = similarity_errors(ba.R.cpu().numpy(), ba.t.cpu().numpy(), Rs, ts)
+    print("global reconstruction of %d views: positioning in %d trial steps (%d CG), %d of %d observations inliers; "
+          "%d tracks triangulated; bundle adjustment in %d trial steps" % (
+              len(Rs), int(gpos.iters[0]), int(gpos.cg_iters[0]), int(gpos.inliers.sum()), int(gpos.n_used[0]),
+              int((tr.n_inliers >= 2).sum()), int(ba.iters[0])))
+    print("  centre error (baseline 0.3): largest %.2e positioned, %.2e adjusted; rotation error: largest %.3f deg "
+          "averaged, %.3f deg adjusted" % (c0.max(), c1.max(), r0.max(), r1.max()))
+    return c0.max(), c1.max(), r1.max()
+
+
+def global_reconstruction(dev, K):
+    """The path scene's 100 views from descriptors to a bundle-adjusted reconstruction, no poses from outside"""
+    scene = path_scene(dev)
+    report_global_reconstruction(scene, global_reconstruction_run(dev, K, scene))
+
+
 def self_calibration(dev, n_img=20, n_pts=4000, seed=9):
     """Views through a lens with radial distortion (f = 520, k1 = -0.08, k2 = 0.01), known tracks, and a start with a
     focal length 5 % off and no distortion: undistort, triangulate, adjust poses, points and the intrinsics of the one
@@ -396,6 +461,7 @@ def main():
     tracks_across_views(dev, K)
     global_adjustment(dev, K)
     rotations_from_view_graph(dev, K)
+    global_reconstruction(dev, K)
     self_calibration(dev)
 
 

@@ -738,6 +738,68 @@ int dgb200_average_rotations_dev(const int32_t* h_pairs, int n_pairs, int n_view
                                  int32_t* d_component_out, double* d_residual_out, int32_t* d_iters_out,
                                  int32_t* d_cg_iters_out, void* stream);
 const char* dgb200_rotation_averaging_last_error(void);
+/* Global positioning (the second step of global SfM, GLOMAP's global positioner with point-to-camera constraints): the
+ * views' centres and the tracks' points from the views' rotations and the tracks' rays.  Translations are not taken.
+ *   Layout: the tracks of dgb200_triangulate_tracks_ragged_dev (d_cams, d_pts, d_offsets [n_tracks + 1], d_mask or
+ *   NULL; the padded output of dgb200_build_tracks_ragged_dev goes in as it is), world-to-camera rotations d_R
+ *   [n_cams][9] (what dgb200_average_rotations_dev returns) and K [9] (k_per_camera as there).
+ *   1 Registered view: R finite with det R > 0.5.  Usable observation: its mask set, its camera in range and registered,
+ *     a finite pixel; its ray v = normalise(R^T K^-1 (x, y, 1)).  Used track: usable observations from at least 2
+ *     distinct cameras; its usable observations are then used.  A track with offsets that decrease, are negative or
+ *     pass `obs` is not used and none of its rows is read.
+ *   2 Components: the connected components of the views over the used tracks; each component's smallest view is its
+ *     anchor, whose centre is held at 0.  A view without a used observation is inactive: t = NaN, component -1.  The
+ *     result is defined up to a similarity per component (the scale is free, as in GLOMAP).
+ *   3 Unknowns: a centre c_i per active view that is not an anchor, a point X_j per used track and a scale d_o per used
+ *     observation, d_o >= d_min = 1e-5.
+ *   4 Cost C = sum_o rho(|r_o|^2), r_o = d_o (X_j - c_i) - v_o (BATA's pairwise direction error); rho(s) = s when
+ *     loss_scale = 0, else the Huber loss of scale delta = loss_scale: s for s <= delta^2, 2 delta sqrt(s) - delta^2
+ *     above.  The normal equations use the IRLS weights w = min(1, delta / |r|) at the linearisation point.
+ *   5 Start: c_i and X_j uniform in [-init_scale, init_scale]^3, all d = 1, anchors at 0.  Coordinate k of view i is
+ *     init_scale (2 u - 1), u = (o[k] + 1/2) 2^-32, o = Philox4x32-10 (csrc/rng.h) of counter (0, i, 0, 0) and key
+ *     (seed low 32 bits, seed high 32 bits); track j's uses counter (0, j, 1, 0).
+ *   6 Schedule, that of dgb200_bundle_adjust_ragged_dev: Levenberg-Marquardt with lambda from 1e-3, a strictly lower
+ *     cost accepts and sets lambda <- max(lambda / 10, 1e-12), otherwise lambda <- 10 lambda; it stops after max_iters
+ *     trial steps, a trial step that changes the cost by less than 1e-12 of it, or lambda > 1e8.  Marquardt damping
+ *     lambda diag(J^T W J) over every coordinate, the scales included.
+ *   7 Trial step by a nested Schur complement.  With a = X - c, u = a / |a|, s = w d^2 and P = I - u u^T / (1 +
+ *     lambda), an observation's scale is eliminated (H_dd* = (1 + lambda) w |a|^2), which leaves m = s P in its
+ *     centre's and its point's blocks (-m between them) and e = w d (r - u (u . r) / (1 + lambda)) in their gradients
+ *     (-e at the centre, +e at the point).  Then each point: V*_j = sum m + lambda sum s I, g_j = sum e, t_j = V*_j^-1
+ *     g_j.  The reduced system over the centres that move, S dc = b with S = U* - sum_j W_j V*_j^-1 W_j^T, U*_i = sum
+ *     m + lambda sum s I, b_i = sum_{o in i} (e_o - m_o t_j), is solved by PCG with the stopping rules of
+ *     dgb200_bundle_adjust_pcg_ragged_dev (x0 = 0; |r| <= cg_tol |b| or cg_max_iters iterations; kappa <= 0 or not
+ *     finite stops, and on the first iteration rejects the step) and the block-Jacobi preconditioner M_i = S_ii = U*_i -
+ *     sum_j W_ij V*_j^-1 W_ij, W_ij the sum of m over view i's observations of track j (3 x 3, Cholesky); anchors and
+ *     inactive views get identity rows.  Back-substitution: dX_j = -t_j + V*_j^-1
+ *     sum m dc_i, dd = -(a . r + d a . (dX - dc)) / ((1 + lambda) |a|^2), trial d <- max(d + dd, d_min).  A non-positive
+ *     pivot of any V* or M rejects the step.  A used observation with |a| = 0 or not finite at the linearisation point
+ *     rejects every step from it (lambda grows until the call stops); at a trial point it costs +inf.
+ * Outputs: d_t_out [n_cams][3] = -R c, so that (R, t) goes straight into triangulation and bundle adjustment;
+ * d_X_out [n_tracks][3] (NaN for a track that is not used); d_component_out int32 [n_cams] the anchor of each view's
+ * component or -1; d_angle_out [obs] the angle between v_o and X_j - c_i at the output, atan2(|v x a|, v . a) (NaN for
+ * an observation that is not used); d_inliers_out uint8 [obs]: used and angle <= max_angle; d_cost0_out [1],
+ * d_cost_out [1] the cost at the start and at the output; d_iters_out [1] the trial steps; d_n_used_out [1] the used
+ * observations; d_cg_iters_out [1] the products S p, summed over the trial steps.
+ * Determinism: no floating-point atomics; every sum is taken in a fixed order over partitions that do not depend on the
+ * launch grid, so a rerun gives the same bytes.  A null required buffer (d_angle_out and d_inliers_out are when obs >
+ * 0), n_tracks < 1, obs < 0, n_cams < 1, loss_scale that is negative or not finite, max_iters < 0 (the shared checks of
+ * the bundle adjustments, in their order), init_scale or max_angle not a non-negative finite number, cg_max_iters < 1
+ * or cg_tol not a non-negative finite number returns DGB200_E_ARG before any launch; the message is
+ * dgb200_global_positioning_last_error()'s.  Asynchronous on `stream`: 4 memsets and 10 launches before the trial
+ * steps, 6 launches per trial step whatever cg_max_iters is (the PCG loop is one cooperative launch sized by the
+ * occupancy API; every kernel returns at once once the call has stopped) and 3 for the outputs, and a stream-ordered
+ * workspace (cudaMallocAsync / cudaFreeAsync) of 161 bytes per observation, 276 bytes per track, 628 bytes per view and
+ * 4 bytes per view and 4096 observations; nothing is read back. */
+int dgb200_global_positioning_ragged_dev(const int32_t* d_cams, const double* d_pts, const double* d_R,
+                                         const double* d_K, int k_per_camera, int n_cams, const int32_t* d_offsets,
+                                         int n_tracks, int obs, const uint8_t* d_mask, uint64_t seed,
+                                         double init_scale, double loss_scale, int max_iters, double max_angle,
+                                         int cg_max_iters, double cg_tol, double* d_t_out, double* d_X_out,
+                                         int32_t* d_component_out, double* d_angle_out, uint8_t* d_inliers_out,
+                                         double* d_cost0_out, double* d_cost_out, int32_t* d_iters_out,
+                                         int32_t* d_n_used_out, int32_t* d_cg_iters_out, void* stream);
+const char* dgb200_global_positioning_last_error(void);
 /* The reference's alternative 7-point null-space solver nullspace_qr7x9 (Ftools.c:594-668, compile-time USE_QR,
  * exp_ranF.c:1346-1349) over `count` systems: d_A [count][7*9] row-major -> d_N [count][2*9], d_rc [count] or NULL. */
 int dgb200_nullspace_qr7x9_batch_dev(const double* d_A, double* d_N, int32_t* d_rc, int count, void* stream);

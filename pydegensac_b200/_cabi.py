@@ -98,6 +98,10 @@ def lib():
         L.dgb200_average_rotations_dev.argtypes = [i32, ci, ci, vp, vp, vp, cd, ci, ci, cd, ci, cd, vp, vp, vp, vp, vp,
                                                    vp]
         L.dgb200_rotation_averaging_last_error.restype = ctypes.c_char_p
+        L.dgb200_global_positioning_ragged_dev.argtypes = [vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, ctypes.c_uint64, cd,
+                                                           cd, ci, cd, ci, cd, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
+                                                           vp]
+        L.dgb200_global_positioning_last_error.restype = ctypes.c_char_p
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p
         L.dgb200_last_error.restype = ctypes.c_char_p

@@ -91,6 +91,8 @@ BundleAdjustmentIntrinsics = collections.namedtuple("BundleAdjustmentIntrinsics"
                                                     "R t X intrinsics mask cost0 cost iters n_used cg_iters")
 TrackSet = collections.namedtuple("TrackSet", "offsets cams kp pts track_of stats")
 RotationAveraging = collections.namedtuple("RotationAveraging", "R component residual iters cg_iters")
+GlobalPositioning = collections.namedtuple("GlobalPositioning",
+                                           "t X component angle inliers cost0 cost iters n_used cg_iters")
 HomographyPose = collections.namedtuple("HomographyPose",
                                         "R t plane good rotation_only points in_front angle median_angle")
 
@@ -1139,6 +1141,75 @@ def average_rotations(pairs, R_rel, n_views, mask=None, weights=None, sigma=math
           pr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), P, n_views, Rr, _mask_u8(mask), w, sigma, l1_iters,
           max_iters, step_tol, cg_max_iters, cg_tol, R, comp, res, iters, cg_iters)
     return RotationAveraging(R, comp, res, iters, cg_iters)
+
+
+def global_positioning_ragged(cams, pts, R, K, offsets, mask=None, seed=0, init_scale=100.0, loss_scale=0.1,
+                              max_iters=100, max_angle=math.radians(2.0), cg_max_iters=500, cg_tol=1e-6):
+    """Position the views and their tracks from the views' rotations: the centre of every view and the point of every
+    track, as global SfM does after rotation averaging (GLOMAP's global positioner with point-to-camera constraints,
+    on the device).  Translations are not taken.
+
+    cams, pts, offsets and mask are CUDA tensors on one device in the layout of triangulate_tracks_ragged (the padded
+    output of build_tracks_ragged goes in as it is); R [C,3,3] the world-to-camera rotations (what average_rotations
+    returns: a view whose R is not finite or whose det R <= 0.5 is not registered); K [3,3] or [C,3,3].  Floating
+    inputs are used in float64.  A track is used when its usable observations come from at least 2 distinct views.
+    Each observation's ray v = normalise(R^T K^-1 (x, y, 1)) constrains its view's centre c and its track's point X
+    through r = d (X - c) - v with a scale d >= 1e-5 of its own; the cost sum rho(|r|^2) uses the Huber loss of scale
+    loss_scale (0: the squared error).  Levenberg-Marquardt from a random start (centres and points uniform in
+    [-init_scale, init_scale]^3 from the Philox stream of `seed`, every d = 1) runs at most max_iters trial steps, each
+    solved by conjugate gradients on the centres (cg_max_iters, cg_tol) once the scales and the points are
+    eliminated.  Each component of the view graph has its smallest view at the origin and a free scale.  max_angle: the
+    largest angle between an observation's ray and its point, in radians, for `inliers`.  The estimator is specified
+    in include/degensac_b200.h.
+    Returns GlobalPositioning(t, X, component, angle, inliers, cost0, cost, iters, n_used, cg_iters): t [C,3] float64 =
+    -R c, so that (R, t) feeds triangulate_tracks_ragged and bundle_adjust_pcg_ragged (NaN for a view without a used
+    observation); X [T,3] (NaN for a track that is not used); component int32 [C] the smallest view of each view's
+    component, or -1; angle [obs] float64 (NaN for an observation that is not used); inliers [obs] bool, the used
+    observations with angle <= max_angle, the mask that triangulation and bundle adjustment take next; cost0, cost [1]
+    float64; iters, n_used, cg_iters [1] int32.  Asynchronous, nothing is read back."""
+    import torch
+    named = (("cams", cams), ("pts", pts), ("R", R), ("K", K), ("offsets", offsets))
+    _check_tensors(named, mask)
+    T = _check_offsets(offsets, "T")
+    _check_int32("cams", cams)
+    obs = _check_columns("pts", pts, "obs", 2)
+    _check_shape("cams", cams, "obs", (obs,))
+    if R.dim() != 3 or R.shape[0] < 1 or tuple(R.shape[1:]) != (3, 3):
+        raise ValueError("R must be [C,3,3] with C >= 1, not %s" % list(R.shape))
+    C = int(R.shape[0])
+    _check_K("K", K, "C", C)
+    _check_floating(named[1:4])
+    _check_mask(mask, "obs", obs)
+    seed = int(seed)
+    if not 0 <= seed < 1 << 64:
+        raise ValueError("seed must lie in [0, 2^64), not %d" % seed)
+    init_scale, loss_scale, max_angle, cg_tol = float(init_scale), float(loss_scale), float(max_angle), float(cg_tol)
+    for nm, v in (("init_scale", init_scale), ("loss_scale", loss_scale), ("max_angle", max_angle)):
+        if not 0.0 <= v < float("inf"):
+            raise ValueError("%s must be a non-negative finite number, not %r" % (nm, v))
+    max_iters = _check_count("max_iters", max_iters, 0)
+    cg_max_iters = _check_count("cg_max_iters", cg_max_iters, 1)
+    if not 0.0 <= cg_tol < float("inf"):
+        raise ValueError("cg_tol must be a non-negative finite number, not %r" % (cg_tol,))
+    dev = _check_device(named, mask)
+    x, Rc, Kc = _f64(pts, R, K)
+    cm, off, m = cams.contiguous(), offsets.contiguous(), _mask_u8(mask)
+    f64, i32 = torch.float64, torch.int32
+    L = _cabi.lib()
+    t = torch.empty((C, 3), dtype=f64, device=dev)
+    X = torch.empty((T, 3), dtype=f64, device=dev)
+    comp = torch.empty(C, dtype=i32, device=dev)
+    ang = torch.empty(max(obs, 1), dtype=f64, device=dev)[:obs]
+    inl = _rows_out(obs, dev)
+    cost0 = torch.empty(1, dtype=f64, device=dev)
+    cost = torch.empty(1, dtype=f64, device=dev)
+    iters = torch.empty(1, dtype=i32, device=dev)
+    n_used = torch.empty(1, dtype=i32, device=dev)
+    cg_iters = torch.empty(1, dtype=i32, device=dev)
+    _call(L.dgb200_global_positioning_ragged_dev, L.dgb200_global_positioning_last_error, dev, cm, x, Rc, Kc,
+          int(Kc.dim() == 3), C, off, T, obs, m, seed, init_scale, loss_scale, max_iters, max_angle, cg_max_iters,
+          cg_tol, t, X, comp, ang, inl, cost0, cost, iters, n_used, cg_iters)
+    return GlobalPositioning(t, X, comp, ang, inl.view(torch.bool), cost0, cost, iters, n_used, cg_iters)
 
 
 def match_descriptors_batch(descs, pairs, kps=None, ratio=0.9, mutual=False, norm="l2"):
