@@ -23,8 +23,8 @@
 //   ba_decide_kernel    one CTA: fixed-order sum of the track costs, accept / reject / stop, lambda, buffer swap.
 // After the last step ba_finish_cameras_kernel and ba_finish_tracks_kernel write the outputs and the inlier mask.
 // No floating-point atomics anywhere: every sum has a fixed order, so a rerun gives the same bytes.  The bodies of the
-// mark, init and finish kernels are in bundle_adjust_device.h and the argument checks in bundle_adjust_args.h, shared
-// with the iterative solver of bundle_adjust_pcg.cu.
+// mark, init, decide and finish kernels are in bundle_adjust_device.h, the argument checks in bundle_adjust_args.h
+// and the launch plumbing in adjust_host.h, shared with the iterative solver of bundle_adjust_pcg.cu.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -39,6 +39,7 @@
 #include "bundle_adjust.h"
 #include "device_util.h"
 #include "bundle_adjust_device.h"
+#include "adjust_host.h"
 
 namespace {
 
@@ -416,34 +417,10 @@ __global__ void __launch_bounds__(kBaThreads) ba_backsub_kernel(BaArgs a) {
   if (lane == 0) a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost] = c;
 }
 
-// The schedule of pose_refine_ragged_kernel on the summed cost
 __global__ void __launch_bounds__(kBaCta) ba_decide_kernel(BaArgs a) {
   __shared__ double shd[kBaCta];
-  BaState* st = a.state;
-  if (st->stop) return;                                // (block-uniform)
-  const bool go = !st->bad;
-  double c = 0.0;
-  if (go)
-    for (int j = threadIdx.x; j < a.n_tracks; j += kBaCta) c += a.trk[dg::kBaTrkStride * (size_t)j + dg::kBaTrkCost];
-  c = block_sum_double(c, shd);                        // (every thread reads st before thread 0 writes it)
-  if (threadIdx.x == 0) {
-    const double c_old = st->cost, c_new = go ? c : c_old;
-    const bool better = go && c_new < c_old;
-    const bool flat = go && fabs(c_old - c_new) < dg::kPrRelDecrease * c_old;
-    st->iters += 1;
-    st->bad = 0;
-    if (better) {
-      st->cost = c_new;
-      st->cur = 1 - st->cur;
-      st->lam = fmax(st->lam / 10.0, dg::kPrLambdaMin);
-      st->lin = 1;
-      if (flat) st->stop = 1;
-    } else {
-      st->lin = 0;
-      st->lam *= 10.0;
-      if (flat || st->lam > dg::kPrLambdaMax) st->stop = 1;
-    }
-  }
+  if (a.state->stop) return;                           // (block-uniform)
+  ba_decide_step(a, shd);
 }
 
 // ---------------------------------------------------------------------------------------------- outputs
@@ -456,13 +433,6 @@ __global__ void __launch_bounds__(kBaThreads) ba_finish_tracks_kernel(BaArgs a) 
   const int j = blockIdx.x * kBaWarps + (threadIdx.x >> 5);
   if (j >= a.n_tracks) return;
   ba_finish_track(a, j, lane);
-}
-
-template <typename T>
-T* carve(char*& p, size_t count) {
-  T* out = (T*)p;
-  p += (sizeof(T) * count + 255) / 256 * 256;
-  return out;
 }
 
 }  // namespace
@@ -489,69 +459,65 @@ int dgb200_bundle_adjust_ragged_dev(const int32_t* d_cams, const double* d_pts, 
   const int n = dg::kBaCamParams * n_free;
   const size_t no = (size_t)(obs > 0 ? obs : 1), nt = (size_t)n_tracks, nc = (size_t)n_cams;
   const size_t nn = (size_t)(n > 0 ? n : 1);
-  const size_t bytes = 256 * 16 + sizeof(double) * (dg::kTrCamStride * nc + 24 * nc + 6 * nt + dg::kBaObsStride * no +
-                                                    dg::kBaTrkStride * nt + nn * nn + nn) +
-                       sizeof(BaState) + sizeof(int) * (nc + 2 * no + 2 * (size_t)n_free + 1 + nt) + 2 * no;
-  char* ws = nullptr;
-  CU(cudaMallocAsync((void**)&ws, bytes, st));
   BaArgs a;
   a.cams = d_cams; a.pts = d_pts; a.R = d_R; a.t = d_t; a.K = d_K; a.k_per_camera = k_per_camera; a.n_cams = n_cams;
   a.offsets = d_offsets; a.mask = d_mask; a.X = d_X; a.n_tracks = n_tracks; a.obs = obs; a.n_free = n_free; a.n = n;
   a.gauge_slot = gauge_slot; a.held_cam = held_cam; a.n_blocks = n_free * (n_free + 1) / 2;
   for (int q = 0; q < dg::kBaMaxFree; ++q) a.free[q] = q < n_free ? h_free[q] : -1;
   a.sig2 = loss_scale * loss_scale; a.th2 = px_th * px_th;
-  char* p = ws;
-  a.tab = carve<double>(p, dg::kTrCamStride * nc);
-  a.poses = carve<double>(p, 24 * nc);
-  a.Xb = carve<double>(p, 6 * nt);
-  a.obsd = carve<double>(p, dg::kBaObsStride * no);
-  a.trk = carve<double>(p, dg::kBaTrkStride * nt);
-  a.S = carve<double>(p, nn * nn);
-  a.rhs = carve<double>(p, nn);
-  a.state = carve<BaState>(p, 1);
-  a.slot_of = carve<int>(p, nc);
-  a.track_of = carve<int>(p, no);
-  a.list = carve<int>(p, no);
-  a.counts = carve<int>(p, n_free + 1);
-  a.list_off = carve<int>(p, n_free + 1);
-  a.trk_used = carve<int>(p, nt);
-  a.usable = carve<unsigned char>(p, no);
-  a.used = carve<unsigned char>(p, no);
+  auto lay_out = [&](char* base) {
+    Carve w{base};
+    a.tab = w.take<double>(dg::kTrCamStride * nc);
+    a.poses = w.take<double>(24 * nc);
+    a.Xb = w.take<double>(6 * nt);
+    a.obsd = w.take<double>(dg::kBaObsStride * no);
+    a.trk = w.take<double>(dg::kBaTrkStride * nt);
+    a.S = w.take<double>(nn * nn);
+    a.rhs = w.take<double>(nn);
+    a.state = w.take<BaState>(1);
+    a.slot_of = w.take<int>(nc);
+    a.track_of = w.take<int>(no);
+    a.list = w.take<int>(no);
+    a.counts = w.take<int>(n_free + 1);
+    a.list_off = w.take<int>(n_free + 1);
+    a.trk_used = w.take<int>(nt);
+    a.usable = w.take<unsigned char>(no);
+    a.used = w.take<unsigned char>(no);
+    return w.bytes;
+  };
+  char* ws = nullptr;
+  const size_t bytes = lay_out(nullptr);
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
+  lay_out(ws);
   a.R_out = d_R_out; a.t_out = d_t_out; a.X_out = d_X_out; a.mask_out = d_mask_out;
   a.cost0_out = d_cost0_out; a.cost_out = d_cost_out; a.iters_out = d_iters_out; a.n_used_out = d_n_used_out;
-  const int cam_grid = (n_cams + kBaCamThreads - 1) / kBaCamThreads;
-  const int trk_grid = (n_tracks + kBaWarps - 1) / kBaWarps;
+  const int cam_grid = blocks(nc, kBaCamThreads);
+  const int trk_grid = blocks(nt, kBaWarps);
   cudaError_t launch = cudaSuccess;
-#define L5(...)                                   \
-  if (launch == cudaSuccess) {                    \
-    __VA_ARGS__;                                  \
-    launch = cudaGetLastError();                  \
-  }
-  L5(launch = cudaMemsetAsync(a.usable, 0, no, st));       // rows outside every span are neither usable nor used
-  L5(launch = cudaMemsetAsync(a.used, 0, no, st));
-  L5(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (n_free + 1), st));
-  L5((ba_cameras_kernel<<<cam_grid, kBaCamThreads, 0, st>>>(a)));
-  L5((ba_mark_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.usable, 0, no, st));   // rows outside every span are neither usable nor used
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.used, 0, no, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (n_free + 1), st));
+  ADJ_LAUNCH((ba_cameras_kernel<<<cam_grid, kBaCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((ba_mark_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
   if (n_free > 0) {
-    L5((ba_count_kernel<<<n_free, kBaCta, 0, st>>>(a)));
-    L5((ba_list_kernel<<<n_free, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_count_kernel<<<n_free, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_list_kernel<<<n_free, kBaCta, 0, st>>>(a)));
   }
-  L5((ba_init_kernel<<<1, kBaCta, 0, st>>>(a)));
-  const int schur_grid = (a.n_blocks + kBaWarps - 1) / kBaWarps;
+  ADJ_LAUNCH((ba_init_kernel<<<1, kBaCta, 0, st>>>(a)));
+  const int schur_grid = blocks((size_t)a.n_blocks, kBaWarps);
   for (int it = 0; it < max_iters && launch == cudaSuccess; ++it) {
-    L5((ba_linearise_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
-    L5((ba_points_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_linearise_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_points_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
     if (n_free > 0) {
-      L5((ba_schur_kernel<<<schur_grid, kBaThreads, 0, st>>>(a)));
-      L5((ba_solve_kernel<<<1, kBaCta, 0, st>>>(a)));
+      ADJ_LAUNCH((ba_schur_kernel<<<schur_grid, kBaThreads, 0, st>>>(a)));
+      ADJ_LAUNCH((ba_solve_kernel<<<1, kBaCta, 0, st>>>(a)));
     }
-    L5((ba_backsub_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
-    L5((ba_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_backsub_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ba_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
   }
-  if (obs > 0) L5(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
-  L5((ba_finish_cameras_kernel<<<cam_grid, kBaCamThreads, 0, st>>>(a)));
-  L5((ba_finish_tracks_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
-#undef L5
+  if (obs > 0) ADJ_LAUNCH(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
+  ADJ_LAUNCH((ba_finish_cameras_kernel<<<cam_grid, kBaCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((ba_finish_tracks_kernel<<<trk_grid, kBaThreads, 0, st>>>(a)));
   CU(cudaFreeAsync(ws, st));
   CU(launch);
   return 0;

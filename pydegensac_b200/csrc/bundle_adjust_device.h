@@ -1,8 +1,7 @@
 // bundle_adjust_device.h -- the kernel bodies that the dense bundle adjustment (bundle_adjust.cu) and the iterative one
 // (bundle_adjust_pcg.cu) share, with the one that also refines the intrinsics (bundle_adjust_intrinsics.cu): the LM
-// state, the fixed-order CTA sums, the counting sort of the observations (bundle_adjust_intrinsics.cu only), the marking
-// of the usable observations and optimised tracks, the start state, the step decision (not bundle_adjust.cu) and the
-// outputs.  Device code, in the anonymous namespace of the
+// state, the fixed-order CTA sums, the counting sort of the observations (not bundle_adjust.cu), the marking of the
+// usable observations and optimised tracks, the start state, the step decision and the outputs.  Device code, in the anonymous namespace of the
 // including translation unit (after device_util.h), as each kernel source keeps its own.
 //
 // The templates take the translation unit's argument block A, which has the members used here with the meaning they
@@ -72,8 +71,7 @@ __device__ double block_sum_double(double v, double* sh) {
 // atomics.  ba_sort_count: the counts; ba_sort_scan (one CTA of kBaCta threads, sh: kBaCta ints): their exclusive
 // prefix sum in key-major order, in place, and list_off [n_keys + 1] the start of each key; ba_sort_scatter: pos_of
 // [obs] the position of each observation in the key-major list, ascending observation order within a key, and item
-// [position] = track_of of its observation.  bundle_adjust_pcg.cu keeps these bodies written out in its pcg_hist,
-// pcg_scan and pcg_scatter kernels: calling them there changes those kernels' register allocation and instructions.
+// [position] = track_of of its observation.
 __device__ __forceinline__ void ba_sort_count(const int* key, int obs, int range, int* hist, int n_ranges, int w,
                                               int lane) {
   const int r0 = w * range, r1 = min(r0 + range, obs);
@@ -235,8 +233,7 @@ __device__ __forceinline__ void ba_init_state(const A& a) {
 }
 
 // One CTA of kBaCta threads (shd: kBaCta doubles of shared memory), once the call has not stopped (the kernel returns
-// first when st->stop): the schedule of pose_refine_ragged_kernel on the summed cost of the tracks.  bundle_adjust.cu
-// keeps this body written out in ba_decide_kernel: inlined there, it compiles to a different branch layout.
+// first when st->stop): the schedule of pose_refine_ragged_kernel on the summed cost of the tracks.
 template <class A>
 __device__ __forceinline__ void ba_decide_step(const A& a, double* shd) {
   BaState* st = a.state;

@@ -39,8 +39,9 @@
 //      list: its share of E_a^T p_a - W_intr,i y (the group's first chunk also adds U*_g p_g), and of p . q;
 //   C  one thread per free slot, one warp per free group (q_g = its chunks' shares in a fixed order): x += alpha p,
 //      r -= alpha q, z = M^-1 r.
-// The dot products are sums of per-slot, per-group and per-chunk terms that every CTA sums itself in one fixed order,
-// so nothing depends on the grid and there are no floating-point atomics: a rerun gives the same bytes.
+// The loop is pcg_run (pcg_device.h).  The dot products are sums of per-slot, per-group and per-chunk terms that every
+// CTA sums itself in one fixed order, so nothing depends on the grid and there are no floating-point atomics: a rerun
+// gives the same bytes.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -57,6 +58,8 @@
 #include "camera_radial.h"
 #include "device_util.h"
 #include "bundle_adjust_device.h"
+#include "pcg_device.h"
+#include "adjust_host.h"
 
 namespace cg = cooperative_groups;
 
@@ -82,15 +85,15 @@ constexpr int kWp = 18, kWk = 15;
 constexpr int kCmW = 0, kCmJc = 18, kCmR = 30, kCmWt = 32, kCmJk = 33, kCm = 43;
 constexpr int kGmW = 0, kGmJk = 15, kGmJc = 25, kGmR = 37, kGmWt = 39, kGm = 40;
 
-// A free slot's record: U (21), g_c (6), L (21), b, x, r, z (6 each), p in two buffers (12), q (6)
-constexpr int kPcU = 0, kPcG = 21, kPcL = 27, kPcB = 48, kPcX = 54, kPcR = 60, kPcZ = 66, kPcP = 72, kPcQ = 84,
-              kPcStride = 90;
-// A free group's record: U (15), g (5), L (15), b, x, r, z (5 each), p in two buffers (10)
-constexpr int kGrU = 0, kGrG = 15, kGrL = 20, kGrB = 35, kGrX = 40, kGrR = 45, kGrZ = 50, kGrP = 55, kGrStride = 65;
+// A free slot's record: U (21), g_c (6), L (21), then its PCG vectors (pcg_device.h): b, x, r, z (6 each), p in two
+// buffers (12), q (6)
+constexpr int kPcU = 0, kPcG = 21, kPcL = 27, kPcB = 48, kPcX = 54, kPcP = 72, kPcQ = 84, kPcStride = 90;
+// A free group's record: U (15), g (5), L (15), then b, x, r, z (5 each), p in two buffers (10); no q, which its chunks
+// hold
+constexpr int kGrU = 0, kGrG = 15, kGrL = 20, kGrB = 35, kGrX = 40, kGrP = 55, kGrStride = 65;
 // A chunk's partials: U (15), g (5), sum W V*^-1 W^T (15), sum W V*^-1 g_p (5); in the PCG loop its q share (5)
 constexpr int kChU = 0, kChG = 15, kChM = 20, kChH = 35, kChStride = 40;
-// The terms of the dot products, kParts arrays of n_part = n_free + n_gfree + chunk capacity entries
-constexpr int kPartPQ = 0, kPartRR = 1, kPartRZ = 2, kPartBB = 3, kParts = 4;
+// The terms of the dot products (pcg_device.h): kPcgParts arrays of n_part = n_free + n_gfree + chunk capacity entries
 
 struct BaiArgs {
   const int* cams; const double* pts;                      // [obs], [obs][2]
@@ -115,7 +118,7 @@ struct BaiArgs {
   double* slot;      // [n_free][kPcStride]
   double* grp;       // [n_gfree][kGrStride]
   double* chk;       // [n_chunks][kChStride]
-  double* part;      // [kParts][n_part]
+  double* part;      // [kPcgParts][n_part]
   BaState* state;
   int* cg_iters;     // [1]
   int* slot_of;      // [n_cams]
@@ -404,23 +407,11 @@ __global__ void __launch_bounds__(kBaiThreads) bai_precond_kernel(BaiArgs a) {
   }
   double z[6];
   dg::pr_cholesky_apply<6>(rec + kPcL, b, z);
-  double rz = 0.0, bb = 0.0;
+  pcg_start<6>(rec + kPcB, b, z, a.part, a.n_part, s);
 #pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    rec[kPcB + k] = b[k];
-    rec[kPcX + k] = 0.0;
-    rec[kPcR + k] = b[k];
-    rec[kPcZ + k] = z[k];
-    rec[kPcP + k] = 0.0;
-    rec[kPcP + 6 + k] = 0.0;
-    rec[kPcG + k] = gc[k];
-    rz += b[k] * z[k];
-    bb += b[k] * b[k];
-  }
+  for (int k = 0; k < 6; ++k) rec[kPcG + k] = gc[k];
 #pragma unroll
   for (int q = 0; q < 21; ++q) rec[kPcU + q] = active ? U[q] : 0.0;
-  part_of(a, kPartRZ)[s] = rz;
-  part_of(a, kPartBB)[s] = bb;
 }
 
 // One warp per chunk of a free group's group-major list: the chunk's partial sums (a fixed tree over the lanes)
@@ -530,58 +521,19 @@ __global__ void __launch_bounds__(kBaiThreads) bai_group_kernel(BaiArgs a) {
   }
   double z[kNK];
   dg::pr_cholesky_apply<kNK>(rec + kGrL, b, z);
-  double rz = 0.0, bb = 0.0;
+  pcg_start<kNK>(rec + kGrB, b, z, a.part, a.n_part, a.n_free + q);
 #pragma unroll
-  for (int k = 0; k < kNK; ++k) {
-    rec[kGrB + k] = b[k];
-    rec[kGrX + k] = 0.0;
-    rec[kGrR + k] = b[k];
-    rec[kGrZ + k] = z[k];
-    rec[kGrP + k] = 0.0;
-    rec[kGrP + kNK + k] = 0.0;
-    rec[kGrG + k] = gg[k];
-    rz += b[k] * z[k];
-    bb += b[k] * b[k];
-  }
+  for (int k = 0; k < kNK; ++k) rec[kGrG + k] = gg[k];
 #pragma unroll
   for (int i = 0; i < kNK2; ++i) rec[kGrU + i] = active ? U[i] : 0.0;
-  part_of(a, kPartRZ)[a.n_free + q] = rz;
-  part_of(a, kPartBB)[a.n_free + q] = bb;
-}
-
-// The fixed-order sums of up to two part arrays of n entries, the same in every CTA: thread t adds entries t,
-// t + kBaiSolveThreads, ... in turn, then a tree over the threads.  Every thread gets the sums.
-__device__ void cta_sum2(const double* u, const double* v, int n, double* sh, double* su, double* sv) {
-  double x = 0.0, y = 0.0;
-  for (int i = threadIdx.x; i < n; i += kBaiSolveThreads) {
-    x += __ldcg(u + i);
-    if (v) y += __ldcg(v + i);
-  }
-  sh[threadIdx.x] = x;
-  sh[kBaiSolveThreads + threadIdx.x] = y;
-  __syncthreads();
-  for (int s = kBaiSolveThreads / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) {
-      sh[threadIdx.x] += sh[threadIdx.x + s];
-      sh[kBaiSolveThreads + threadIdx.x] += sh[kBaiSolveThreads + threadIdx.x + s];
-    }
-    __syncthreads();
-  }
-  *su = sh[0];
-  *sv = sh[kBaiSolveThreads];
-  __syncthreads();
 }
 
 // p = z + beta p' of slot s / free group q, p' in buffer `prev`
 __device__ __forceinline__ void direction(const BaiArgs& a, int s, int prev, double beta, double* p) {
-  const double* rec = slot_rec(a, s);
-#pragma unroll
-  for (int k = 0; k < 6; ++k) p[k] = __ldcg(rec + kPcZ + k) + beta * __ldcg(rec + kPcP + 6 * prev + k);
+  pcg_direction<6>(slot_rec(a, s) + kPcB, prev, beta, p);
 }
 __device__ __forceinline__ void gdirection(const BaiArgs& a, int q, int prev, double beta, double* p) {
-  const double* rec = grp_rec(a, q);
-#pragma unroll
-  for (int k = 0; k < kNK; ++k) p[k] = __ldcg(rec + kGrZ + k) + beta * __ldcg(rec + kGrP + kNK * prev + k);
+  pcg_direction<kNK>(grp_rec(a, q) + kGrB, prev, beta, p);
 }
 
 // U* p of a packed upper triangle U [n (n + 1) / 2], damped on the diagonal
@@ -597,236 +549,206 @@ __device__ __forceinline__ double damped_row(const double* U, double lam, const 
   return v + lam * __ldcg(U + d) * p[k];
 }
 
-// The PCG loop of one trial step, then the trial poses and intrinsics.  Data written inside the launch is read with
-// __ldcg (L2); every CTA computes the same scalars, so every CTA takes the same branches and meets the same grid.sync().
+// pcg_run's S p and phase C over [free slots; free groups].  product: A, one thread per track, y_p = V*_p^-1
+// sum_i (W_pose,i^T p_s(i) + W_intr,i^T p_g(i)); grid.sync; B, one warp per free slot, then one per chunk.  update:
+// one thread per free slot, one warp per free group.
+struct BaiSchur {
+  const BaiArgs& a;
+  int tid, nthr, lane, warp, nwarps;
+  double lam;
+  int hold_row;
+
+  __device__ __forceinline__ void product(cg::grid_group& grid, int cur, int prev, double beta) const {
+    const int nf = a.n_free, ng = a.n_gfree;
+    const size_t no = (size_t)a.obs;
+    for (int j = tid; j < a.n_tracks; j += nthr) {
+      if (a.trk_used[j] == 0) continue;
+      const int b = a.offsets[j], e = a.offsets[j + 1];
+      double u[3] = {0.0, 0.0, 0.0};
+      for (int r = b; r < e; ++r) {
+        const int s = a.sl[r], q = a.gsl[r];
+        if (s >= 0) {
+          double p[6];
+          direction(a, s, prev, beta, p);
+#pragma unroll
+          for (int k = 0; k < 6; ++k)
+#pragma unroll
+            for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wo + (3 * k + m) * no + r) * p[k];
+        }
+        if (q >= 0) {
+          double p[kNK];
+          gdirection(a, q, prev, beta, p);
+#pragma unroll
+          for (int k = 0; k < kNK; ++k)
+#pragma unroll
+            for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wo + (kWp + 3 * k + m) * no + r) * p[k];
+        }
+      }
+      double yv[3];
+      dg::ba_sym3_mul(a.trk + dg::kBaTrkStride * (size_t)j + dg::kBaTrkVi, u, yv);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
+    }
+    grid.sync();
+    for (int v = warp; v < nf + a.n_chunks; v += nwarps) {
+      if (v < nf) {
+        const int s = v;
+        const bool active = a.list_off[s + 1] > a.list_off[s];
+        const int gq = active ? a.gslot_of[a.groups[a.free[s]]] : -1;   // (an active slot's group is valid)
+        double pg[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
+        if (gq >= 0) gdirection(a, gq, prev, beta, pg);
+        double acc[6] = {0, 0, 0, 0, 0, 0};
+        const int i0 = a.list_off[s], i1 = a.list_off[s + 1];
+        for (int i = i0 + lane; i < i1; i += 32) {
+          const double* C = a.Cm + i;
+          const double* yp = a.y + 3 * (size_t)a.ctrk[i];
+          const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
+          // E_a p_g: w J_cam^T (J_intr p_g)
+          double e0 = 0.0, e1 = 0.0;
+          if (gq >= 0) {
+#pragma unroll
+            for (int k = 0; k < kNK; ++k) {
+              e0 += __ldg(C + (kCmJk + k) * no) * pg[k];
+              e1 += __ldg(C + (kCmJk + 5 + k) * no) * pg[k];
+            }
+            const double w = __ldg(C + kCmWt * no);
+            e0 *= w;
+            e1 *= w;
+          }
+#pragma unroll
+          for (int k = 0; k < 6; ++k)
+            acc[k] += __ldg(C + (kCmW + 3 * k) * no) * y0 + __ldg(C + (kCmW + 3 * k + 1) * no) * y1 +
+                      __ldg(C + (kCmW + 3 * k + 2) * no) * y2 -
+                      (__ldg(C + (kCmJc + k) * no) * e0 + __ldg(C + (kCmJc + 6 + k) * no) * e1);
+        }
+#pragma unroll
+        for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
+        if (lane == 0) {
+          double p[6];
+          direction(a, s, prev, beta, p);
+          double* rec = slot_rec(a, s);
+          const int hold = hold_row - dg::kBaCamParams * s;
+          double pq = 0.0;
+#pragma unroll
+          for (int k = 0; k < 6; ++k) {
+            double q = damped_row<6>(rec + kPcU, lam, p, k) - acc[k];
+            if (k == hold) q = p[k];
+            rec[kPcQ + k] = q;
+            rec[kPcP + 6 * cur + k] = p[k];
+            pq += p[k] * q;
+          }
+          part_of(a, kPartPQ)[s] = pq;
+        }
+      } else {
+        const int c = v - nf;
+        if (c >= a.chunk_off[ng]) continue;          // past the last chunk (warp-uniform)
+        int lo = 0, hi = ng - 1;
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) >> 1;
+          if (a.chunk_off[mid] <= c) lo = mid; else hi = mid - 1;
+        }
+        const int q = lo, i0 = a.chunk_beg[c], i1 = chunk_end(a, q, c);
+        double pg[kNK];
+        gdirection(a, q, prev, beta, pg);
+        double acc[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
+        for (int i = i0 + lane; i < i1; i += 32) {
+          const double* G = a.Gm + i;
+          const double* yp = a.y + 3 * (size_t)a.gtrk[i];
+          const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
+          const int s = a.gcs[i];
+          double e0 = 0.0, e1 = 0.0;
+          if (s >= 0) {                              // E_a^T p_a: w J_intr^T (J_cam p_a)
+            double p[6];
+            direction(a, s, prev, beta, p);
+#pragma unroll
+            for (int k = 0; k < 6; ++k) {
+              e0 += __ldg(G + (kGmJc + k) * no) * p[k];
+              e1 += __ldg(G + (kGmJc + 6 + k) * no) * p[k];
+            }
+            const double w = __ldg(G + kGmWt * no);
+            e0 *= w;
+            e1 *= w;
+          }
+#pragma unroll
+          for (int k = 0; k < kNK; ++k)
+            acc[k] += __ldg(G + (kGmJk + k) * no) * e0 + __ldg(G + (kGmJk + 5 + k) * no) * e1 -
+                      (__ldg(G + (kGmW + 3 * k) * no) * y0 + __ldg(G + (kGmW + 3 * k + 1) * no) * y1 +
+                       __ldg(G + (kGmW + 3 * k + 2) * no) * y2);
+        }
+#pragma unroll
+        for (int k = 0; k < kNK; ++k) acc[k] = warp_sum(acc[k]);
+        if (lane == 0) {
+          const double* rec = grp_rec(a, q);
+          const bool first = c == a.chunk_off[q];
+          double* ch = a.chk + kChStride * (size_t)c;
+          double pq = 0.0;
+#pragma unroll
+          for (int k = 0; k < kNK; ++k) {
+            double v = acc[k] + (first ? damped_row<kNK>(rec + kGrU, lam, pg, k) : 0.0);
+            if (!refined(a.refine, k)) v = 0.0;      // (p_g is 0 there: q_g = p_g)
+            ch[k] = v;
+            pq += pg[k] * v;
+          }
+          part_of(a, kPartPQ)[nf + ng + c] = pq;
+        }
+      }
+    }
+  }
+
+  __device__ __forceinline__ void update(int cur, int prev, double beta, double alpha) const {
+    const int nf = a.n_free, ng = a.n_gfree;
+    for (int v = tid; v < nf; v += nthr) {
+      double* rec = slot_rec(a, v);
+      double p[6], q[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) {
+        p[k] = __ldcg(rec + kPcP + 6 * cur + k);
+        q[k] = __ldcg(rec + kPcQ + k);
+      }
+      const double2 rz = pcg_update<6>(rec + kPcB, p, q, alpha, [rec](const double* r, double* z) {
+        dg::pr_cholesky_apply<6>(rec + kPcL, r, z);
+      });
+      part_of(a, kPartRR)[v] = rz.x;
+      part_of(a, kPartRZ)[v] = rz.y;
+    }
+    // one warp per free group: q_g = its chunks' shares summed in a fixed order (lane l takes chunks l, l + 32, ...,
+    // then a fixed tree), then x, r, z as for a slot
+    for (int q = warp; q < ng; q += nwarps) {
+      double qv[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
+      for (int c = a.chunk_off[q] + lane; c < a.chunk_off[q + 1]; c += 32)
+#pragma unroll
+        for (int k = 0; k < kNK; ++k) qv[k] += __ldcg(a.chk + kChStride * (size_t)c + k);
+#pragma unroll
+      for (int k = 0; k < kNK; ++k) qv[k] = warp_sum(qv[k]);
+      if (lane == 0) {
+        double* rec = grp_rec(a, q);
+        double p[kNK];
+        gdirection(a, q, prev, beta, p);
+#pragma unroll
+        for (int k = 0; k < kNK; ++k) rec[kGrP + kNK * cur + k] = p[k];
+        const double2 rz = pcg_update<kNK>(rec + kGrB, p, qv, alpha, [rec](const double* r, double* z) {
+          dg::pr_cholesky_apply<kNK>(rec + kGrL, r, z);
+        });
+        part_of(a, kPartRR)[nf + q] = rz.x;
+        part_of(a, kPartRZ)[nf + q] = rz.y;
+      }
+    }
+  }
+};
+
+// The PCG loop of one trial step (pcg_run), then the trial poses and intrinsics
 __global__ void __launch_bounds__(kBaiSolveThreads) bai_solve_kernel(BaiArgs a) {
   __shared__ double sh[2 * kBaiSolveThreads];
   BaState* st = a.state;
   if (st->stop || st->bad) return;                     // (grid-uniform: nothing below writes them before a grid.sync)
   cg::grid_group grid = cg::this_grid();
   const int tid = blockIdx.x * kBaiSolveThreads + threadIdx.x, nthr = gridDim.x * kBaiSolveThreads;
-  const int lane = threadIdx.x & 31, warp = tid >> 5, nwarps = nthr >> 5;
-  const int nf = a.n_free, ng = a.n_gfree, np = a.n_part;
-  const size_t no = (size_t)a.obs;
-  const double lam = st->lam;
-  const int hold_row = st->hold_row;
-  double bb, rho;
-  cta_sum2(part_of(a, kPartBB), part_of(a, kPartRZ), np, sh, &bb, &rho);
-  int it = 0;
-  bool reject = false;
-  if (bb > 0.0) {
-    double beta = 0.0;
-    for (;;) {
-      const int cur = it & 1, prev = cur ^ 1;
-      // A: y_p = V*_p^-1 sum_i (W_pose,i^T p_s(i) + W_intr,i^T p_g(i))
-      for (int j = tid; j < a.n_tracks; j += nthr) {
-        if (a.trk_used[j] == 0) continue;
-        const int b = a.offsets[j], e = a.offsets[j + 1];
-        double u[3] = {0.0, 0.0, 0.0};
-        for (int r = b; r < e; ++r) {
-          const int s = a.sl[r], q = a.gsl[r];
-          if (s >= 0) {
-            double p[6];
-            direction(a, s, prev, beta, p);
-#pragma unroll
-            for (int k = 0; k < 6; ++k)
-#pragma unroll
-              for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wo + (3 * k + m) * no + r) * p[k];
-          }
-          if (q >= 0) {
-            double p[kNK];
-            gdirection(a, q, prev, beta, p);
-#pragma unroll
-            for (int k = 0; k < kNK; ++k)
-#pragma unroll
-              for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wo + (kWp + 3 * k + m) * no + r) * p[k];
-          }
-        }
-        double yv[3];
-        dg::ba_sym3_mul(a.trk + dg::kBaTrkStride * (size_t)j + dg::kBaTrkVi, u, yv);
-#pragma unroll
-        for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
-      }
-      grid.sync();
-      // B: one warp per free slot, then one per chunk
-      for (int v = warp; v < nf + a.n_chunks; v += nwarps) {
-        if (v < nf) {
-          const int s = v;
-          const bool active = a.list_off[s + 1] > a.list_off[s];
-          const int gq = active ? a.gslot_of[a.groups[a.free[s]]] : -1;   // (an active slot's group is valid)
-          double pg[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
-          if (gq >= 0) gdirection(a, gq, prev, beta, pg);
-          double acc[6] = {0, 0, 0, 0, 0, 0};
-          const int i0 = a.list_off[s], i1 = a.list_off[s + 1];
-          for (int i = i0 + lane; i < i1; i += 32) {
-            const double* C = a.Cm + i;
-            const double* yp = a.y + 3 * (size_t)a.ctrk[i];
-            const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
-            // E_a p_g: w J_cam^T (J_intr p_g)
-            double e0 = 0.0, e1 = 0.0;
-            if (gq >= 0) {
-#pragma unroll
-              for (int k = 0; k < kNK; ++k) {
-                e0 += __ldg(C + (kCmJk + k) * no) * pg[k];
-                e1 += __ldg(C + (kCmJk + 5 + k) * no) * pg[k];
-              }
-              const double w = __ldg(C + kCmWt * no);
-              e0 *= w;
-              e1 *= w;
-            }
-#pragma unroll
-            for (int k = 0; k < 6; ++k)
-              acc[k] += __ldg(C + (kCmW + 3 * k) * no) * y0 + __ldg(C + (kCmW + 3 * k + 1) * no) * y1 +
-                        __ldg(C + (kCmW + 3 * k + 2) * no) * y2 -
-                        (__ldg(C + (kCmJc + k) * no) * e0 + __ldg(C + (kCmJc + 6 + k) * no) * e1);
-          }
-#pragma unroll
-          for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
-          if (lane == 0) {
-            double p[6];
-            direction(a, s, prev, beta, p);
-            double* rec = slot_rec(a, s);
-            const int hold = hold_row - dg::kBaCamParams * s;
-            double pq = 0.0;
-#pragma unroll
-            for (int k = 0; k < 6; ++k) {
-              double q = damped_row<6>(rec + kPcU, lam, p, k) - acc[k];
-              if (k == hold) q = p[k];
-              rec[kPcQ + k] = q;
-              rec[kPcP + 6 * cur + k] = p[k];
-              pq += p[k] * q;
-            }
-            part_of(a, kPartPQ)[s] = pq;
-          }
-        } else {
-          const int c = v - nf;
-          if (c >= a.chunk_off[ng]) continue;          // past the last chunk (warp-uniform)
-          int lo = 0, hi = ng - 1;
-          while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if (a.chunk_off[mid] <= c) lo = mid; else hi = mid - 1;
-          }
-          const int q = lo, i0 = a.chunk_beg[c], i1 = chunk_end(a, q, c);
-          double pg[kNK];
-          gdirection(a, q, prev, beta, pg);
-          double acc[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
-          for (int i = i0 + lane; i < i1; i += 32) {
-            const double* G = a.Gm + i;
-            const double* yp = a.y + 3 * (size_t)a.gtrk[i];
-            const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
-            const int s = a.gcs[i];
-            double e0 = 0.0, e1 = 0.0;
-            if (s >= 0) {                              // E_a^T p_a: w J_intr^T (J_cam p_a)
-              double p[6];
-              direction(a, s, prev, beta, p);
-#pragma unroll
-              for (int k = 0; k < 6; ++k) {
-                e0 += __ldg(G + (kGmJc + k) * no) * p[k];
-                e1 += __ldg(G + (kGmJc + 6 + k) * no) * p[k];
-              }
-              const double w = __ldg(G + kGmWt * no);
-              e0 *= w;
-              e1 *= w;
-            }
-#pragma unroll
-            for (int k = 0; k < kNK; ++k)
-              acc[k] += __ldg(G + (kGmJk + k) * no) * e0 + __ldg(G + (kGmJk + 5 + k) * no) * e1 -
-                        (__ldg(G + (kGmW + 3 * k) * no) * y0 + __ldg(G + (kGmW + 3 * k + 1) * no) * y1 +
-                         __ldg(G + (kGmW + 3 * k + 2) * no) * y2);
-          }
-#pragma unroll
-          for (int k = 0; k < kNK; ++k) acc[k] = warp_sum(acc[k]);
-          if (lane == 0) {
-            const double* rec = grp_rec(a, q);
-            const bool first = c == a.chunk_off[q];
-            double* ch = a.chk + kChStride * (size_t)c;
-            double pq = 0.0;
-#pragma unroll
-            for (int k = 0; k < kNK; ++k) {
-              double v = acc[k] + (first ? damped_row<kNK>(rec + kGrU, lam, pg, k) : 0.0);
-              if (!refined(a.refine, k)) v = 0.0;      // (p_g is 0 there: q_g = p_g)
-              ch[k] = v;
-              pq += pg[k] * v;
-            }
-            part_of(a, kPartPQ)[nf + ng + c] = pq;
-          }
-        }
-      }
-      grid.sync();
-      // C: alpha, x, r, z
-      double kappa, unused;
-      cta_sum2(part_of(a, kPartPQ), nullptr, np, sh, &kappa, &unused);
-      ++it;
-      if (!(kappa > 0.0) || !finite(kappa)) {
-        reject = it == 1;
-        break;
-      }
-      const double alpha = rho / kappa;
-      for (int v = tid; v < nf; v += nthr) {
-        double rr = 0.0, rz = 0.0;
-        {
-          double* rec = slot_rec(a, v);
-          double r[6], z[6];
-#pragma unroll
-          for (int k = 0; k < 6; ++k) {
-            rec[kPcX + k] = __ldcg(rec + kPcX + k) + alpha * __ldcg(rec + kPcP + 6 * cur + k);
-            r[k] = __ldcg(rec + kPcR + k) - alpha * __ldcg(rec + kPcQ + k);
-          }
-          dg::pr_cholesky_apply<6>(rec + kPcL, r, z);
-#pragma unroll
-          for (int k = 0; k < 6; ++k) {
-            rec[kPcR + k] = r[k];
-            rec[kPcZ + k] = z[k];
-            rr += r[k] * r[k];
-            rz += r[k] * z[k];
-          }
-        }
-        part_of(a, kPartRR)[v] = rr;
-        part_of(a, kPartRZ)[v] = rz;
-      }
-      // one warp per free group: q_g = its chunks' shares summed in a fixed order (lane l takes chunks l, l + 32, ...,
-      // then a fixed tree), then x, r, z as for a slot
-      for (int q = warp; q < ng; q += nwarps) {
-        double qv[kNK] = {0.0, 0.0, 0.0, 0.0, 0.0};
-        for (int c = a.chunk_off[q] + lane; c < a.chunk_off[q + 1]; c += 32)
-#pragma unroll
-          for (int k = 0; k < kNK; ++k) qv[k] += __ldcg(a.chk + kChStride * (size_t)c + k);
-#pragma unroll
-        for (int k = 0; k < kNK; ++k) qv[k] = warp_sum(qv[k]);
-        if (lane == 0) {
-          double rr = 0.0, rz = 0.0;
-          double* rec = grp_rec(a, q);
-          double p[kNK], r[kNK], z[kNK];
-          gdirection(a, q, prev, beta, p);
-#pragma unroll
-          for (int k = 0; k < kNK; ++k) {
-            rec[kGrP + kNK * cur + k] = p[k];
-            rec[kGrX + k] = __ldcg(rec + kGrX + k) + alpha * p[k];
-            r[k] = __ldcg(rec + kGrR + k) - alpha * qv[k];
-          }
-          dg::pr_cholesky_apply<kNK>(rec + kGrL, r, z);
-#pragma unroll
-          for (int k = 0; k < kNK; ++k) {
-            rec[kGrR + k] = r[k];
-            rec[kGrZ + k] = z[k];
-            rr += r[k] * r[k];
-            rz += r[k] * z[k];
-          }
-          part_of(a, kPartRR)[nf + q] = rr;
-          part_of(a, kPartRZ)[nf + q] = rz;
-        }
-      }
-      grid.sync();
-      double rr, rz;
-      cta_sum2(part_of(a, kPartRR), part_of(a, kPartRZ), np, sh, &rr, &rz);
-      if (rr <= a.cg_tol2 * bb || it >= a.cg_max_iters) break;
-      beta = rz / rho;
-      rho = rz;
-    }
-  }
+  const int nf = a.n_free, ng = a.n_gfree;
+  const BaiSchur op{a, tid, nthr, (int)threadIdx.x & 31, tid >> 5, nthr >> 5, st->lam, st->hold_row};
+  const PcgResult res = pcg_run<kBaiSolveThreads>(grid, a.part, a.n_part, a.cg_tol2, a.cg_max_iters, sh, op);
   // the trial poses and intrinsics (x was last written in a phase C that a grid.sync has closed)
   const int cur = st->cur;
-  if (!reject)
+  if (!res.reject)
     for (int v = tid; v < nf + ng; v += nthr) {
       if (v < nf) {
         if (a.list_off[v + 1] == a.list_off[v]) continue;
@@ -847,8 +769,8 @@ __global__ void __launch_bounds__(kBaiSolveThreads) bai_solve_kernel(BaiArgs a) 
       }
     }
   if (tid == 0) {
-    a.cg_iters[0] += it;
-    if (reject) st->bad = 1;
+    a.cg_iters[0] += res.iters;
+    if (res.reject) st->bad = 1;
   }
 }
 
@@ -939,15 +861,6 @@ __global__ void __launch_bounds__(kBaiCamThreads) undistort_kernel(const double*
   out[2 * (size_t)r + 1] = o[1];
 }
 
-template <typename T>
-T* carve(char*& p, size_t count) {
-  T* out = (T*)p;
-  p += (sizeof(T) * count + 255) / 256 * 256;
-  return out;
-}
-
-int blocks(size_t n, int per) { return (int)((n + per - 1) / per); }
-
 }  // namespace
 
 extern "C" {
@@ -987,11 +900,9 @@ int dgb200_bundle_adjust_intrinsics_ragged_dev(
   if (refine & ~(DGB200_REFINE_FOCAL | DGB200_REFINE_PRINCIPAL_POINT | DGB200_REFINE_DISTORTION))
     return fail(DGB200_E_ARG, "refine must be a set of DGB200_REFINE_* bits");
   const cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  CU(cudaGetDevice(&dev));
-  CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) return fail(DGB200_E_CUDA, "the device does not support cooperative launches");
+  int sms = 0, per_sm = 0;
+  cudaError_t e = cudaSuccess;
+  if (const char* m = coop_sms(&sms, &e)) return fail(DGB200_E_CUDA, m, e);
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, bai_solve_kernel, kBaiSolveThreads, 0));
   if (per_sm < 1) return fail(DGB200_E_CUDA, "bai_solve_kernel does not fit on an SM");
   // a free group with no refined coordinate changes nothing: no group is free then
@@ -1002,19 +913,6 @@ int dgb200_bundle_adjust_intrinsics_ragged_dev(
   const size_t nch = (size_t)obs / kBaiChunk + nq;    // chunks at most: sum over groups of ceil(n_q / kBaiChunk)
   const size_t npart = (size_t)n_free + (size_t)ngf + nch;
   const size_t nkey = nf > nq ? nf : nq;
-  size_t bytes = 0;
-  {                                                    // the carve below, counted
-    const size_t d = sizeof(double), i = sizeof(int);
-    const size_t sizes[] = {d * dg::kTrCamStride * nc, d * 24 * nc, d * 2 * kNK * ng, d * 6 * nt,
-                            d * dg::kBaTrkStride * nt, d * 3 * nt, d * (kWp + kWk) * no, d * kCm * no, d * kGm * no,
-                            d * kPcStride * nf, d * kGrStride * nq, d * kChStride * nch, d * kParts * npart,
-                            sizeof(BaState), i, i * nf, i * nq, i * nc, i * ng, i * no, i * no, i * no, i * no,
-                            i * no, i * no, i * no, i * no, i * nkey * (size_t)n_ranges, i * (nf + 1), i * (nq + 1),
-                            i * (nq + 1), i * nch, i * nt, no, no};
-    for (size_t s : sizes) bytes += (s + 255) / 256 * 256;
-  }
-  char* ws = nullptr;
-  CU(cudaMallocAsync((void**)&ws, bytes, st));
   BaiArgs a;
   a.cams = d_cams; a.pts = d_pts; a.R = d_R; a.t = d_t; a.groups = d_groups; a.intr_in = d_intrinsics;
   a.n_cams = n_cams; a.n_groups = n_groups; a.offsets = d_offsets; a.mask = d_mask; a.X = d_X;
@@ -1022,42 +920,50 @@ int dgb200_bundle_adjust_intrinsics_ragged_dev(
   a.gauge_slot = gauge_slot; a.held_cam = held_cam; a.n_ranges = n_ranges; a.n_chunks = (int)nch;
   a.n_part = (int)npart; a.cg_max_iters = cg_max_iters;
   a.sig2 = loss_scale * loss_scale; a.th2 = px_th * px_th; a.cg_tol2 = cg_tol * cg_tol;
-  char* p = ws;
-  a.tab = carve<double>(p, dg::kTrCamStride * nc);
-  a.poses = carve<double>(p, 24 * nc);
-  a.intr = carve<double>(p, 2 * kNK * ng);
-  a.Xb = carve<double>(p, 6 * nt);
-  a.trk = carve<double>(p, dg::kBaTrkStride * nt);
-  a.y = carve<double>(p, 3 * nt);
-  a.Wo = carve<double>(p, (kWp + kWk) * no);
-  a.Cm = carve<double>(p, kCm * no);
-  a.Gm = carve<double>(p, kGm * no);
-  a.slot = carve<double>(p, kPcStride * nf);
-  a.grp = carve<double>(p, kGrStride * nq);
-  a.chk = carve<double>(p, kChStride * nch);
-  a.part = carve<double>(p, kParts * npart);
-  a.state = carve<BaState>(p, 1);
-  a.cg_iters = carve<int>(p, 1);
-  int* d_free = carve<int>(p, nf);
-  int* d_gfree = carve<int>(p, nq);
-  a.slot_of = carve<int>(p, nc);
-  a.gslot_of = carve<int>(p, ng);
-  a.track_of = carve<int>(p, no);
-  a.sl = carve<int>(p, no);
-  a.gsl = carve<int>(p, no);
-  a.pos_of = carve<int>(p, no);
-  a.gpos_of = carve<int>(p, no);
-  a.ctrk = carve<int>(p, no);
-  a.gtrk = carve<int>(p, no);
-  a.gcs = carve<int>(p, no);
-  a.hist = carve<int>(p, nkey * (size_t)n_ranges);
-  a.list_off = carve<int>(p, nf + 1);
-  a.glist_off = carve<int>(p, nq + 1);
-  a.chunk_off = carve<int>(p, nq + 1);
-  a.chunk_beg = carve<int>(p, nch);
-  a.trk_used = carve<int>(p, nt);
-  a.usable = carve<unsigned char>(p, no);
-  a.used = carve<unsigned char>(p, no);
+  int *d_free = nullptr, *d_gfree = nullptr;
+  auto lay_out = [&](char* base) {
+    Carve w{base};
+    a.tab = w.take<double>(dg::kTrCamStride * nc);
+    a.poses = w.take<double>(24 * nc);
+    a.intr = w.take<double>(2 * kNK * ng);
+    a.Xb = w.take<double>(6 * nt);
+    a.trk = w.take<double>(dg::kBaTrkStride * nt);
+    a.y = w.take<double>(3 * nt);
+    a.Wo = w.take<double>((kWp + kWk) * no);
+    a.Cm = w.take<double>(kCm * no);
+    a.Gm = w.take<double>(kGm * no);
+    a.slot = w.take<double>(kPcStride * nf);
+    a.grp = w.take<double>(kGrStride * nq);
+    a.chk = w.take<double>(kChStride * nch);
+    a.part = w.take<double>(kPcgParts * npart);
+    a.state = w.take<BaState>(1);
+    a.cg_iters = w.take<int>(1);
+    d_free = w.take<int>(nf);
+    d_gfree = w.take<int>(nq);
+    a.slot_of = w.take<int>(nc);
+    a.gslot_of = w.take<int>(ng);
+    a.track_of = w.take<int>(no);
+    a.sl = w.take<int>(no);
+    a.gsl = w.take<int>(no);
+    a.pos_of = w.take<int>(no);
+    a.gpos_of = w.take<int>(no);
+    a.ctrk = w.take<int>(no);
+    a.gtrk = w.take<int>(no);
+    a.gcs = w.take<int>(no);
+    a.hist = w.take<int>(nkey * (size_t)n_ranges);
+    a.list_off = w.take<int>(nf + 1);
+    a.glist_off = w.take<int>(nq + 1);
+    a.chunk_off = w.take<int>(nq + 1);
+    a.chunk_beg = w.take<int>(nch);
+    a.trk_used = w.take<int>(nt);
+    a.usable = w.take<unsigned char>(no);
+    a.used = w.take<unsigned char>(no);
+    return w.bytes;
+  };
+  char* ws = nullptr;
+  const size_t bytes = lay_out(nullptr);
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
+  lay_out(ws);
   a.free = d_free; a.gfree = d_gfree;
   a.R_out = d_R_out; a.t_out = d_t_out; a.X_out = d_X_out; a.intr_out = d_intrinsics_out; a.mask_out = d_mask_out;
   a.cost0_out = d_cost0_out; a.cost_out = d_cost_out; a.iters_out = d_iters_out; a.n_used_out = d_n_used_out;
@@ -1069,59 +975,55 @@ int dgb200_bundle_adjust_intrinsics_ragged_dev(
   const size_t hist_bytes = sizeof(int) * nkey * (size_t)n_ranges;
   void* solve_args[] = {&a};
   cudaError_t launch = cudaSuccess;
-#define L8(...)                                   \
-  if (launch == cudaSuccess) {                    \
-    __VA_ARGS__;                                  \
-    launch = cudaGetLastError();                  \
-  }
-  if (n_free > 0) L8(launch = cudaMemcpyAsync(d_free, h_free, sizeof(int) * (size_t)n_free, cudaMemcpyHostToDevice, st));
+  if (n_free > 0)
+    ADJ_LAUNCH(launch = cudaMemcpyAsync(d_free, h_free, sizeof(int) * (size_t)n_free, cudaMemcpyHostToDevice, st));
   if (ngf > 0)
-    L8(launch = cudaMemcpyAsync(d_gfree, h_free_groups, sizeof(int) * (size_t)ngf, cudaMemcpyHostToDevice, st));
-  L8(launch = cudaMemsetAsync(a.usable, 0, no, st));       // rows outside every span are neither usable nor used
-  L8(launch = cudaMemsetAsync(a.used, 0, no, st));
-  L8(launch = cudaMemsetAsync(a.slot_of, 0xff, sizeof(int) * nc, st));
-  L8(launch = cudaMemsetAsync(a.gslot_of, 0xff, sizeof(int) * ng, st));
-  L8(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nf + 1), st));
-  L8(launch = cudaMemsetAsync(a.glist_off, 0, sizeof(int) * (nq + 1), st));
-  L8(launch = cudaMemsetAsync(a.chunk_off, 0, sizeof(int) * (nq + 1), st));
-  L8(launch = cudaMemsetAsync(a.part, 0, sizeof(double) * kParts * npart, st));   // entries no one writes stay 0
-  L8((bai_cameras_kernel<<<blocks(nc, kBaiCamThreads), kBaiCamThreads, 0, st>>>(a)));
-  L8((bai_slots_kernel<<<cam_grid, kBaiCamThreads, 0, st>>>(a)));
-  L8((bai_mark_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
-  if (obs > 0) L8((bai_slot_obs_kernel<<<obs_grid, kBaiCamThreads, 0, st>>>(a)));
+    ADJ_LAUNCH(launch = cudaMemcpyAsync(d_gfree, h_free_groups, sizeof(int) * (size_t)ngf, cudaMemcpyHostToDevice, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.usable, 0, no, st));   // rows outside every span are neither usable nor used
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.used, 0, no, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.slot_of, 0xff, sizeof(int) * nc, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.gslot_of, 0xff, sizeof(int) * ng, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nf + 1), st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.glist_off, 0, sizeof(int) * (nq + 1), st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.chunk_off, 0, sizeof(int) * (nq + 1), st));
+  // entries no one writes stay 0
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.part, 0, sizeof(double) * kPcgParts * npart, st));
+  ADJ_LAUNCH((bai_cameras_kernel<<<blocks(nc, kBaiCamThreads), kBaiCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((bai_slots_kernel<<<cam_grid, kBaiCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((bai_mark_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
+  if (obs > 0) ADJ_LAUNCH((bai_slot_obs_kernel<<<obs_grid, kBaiCamThreads, 0, st>>>(a)));
   if (n_free > 0 && obs > 0) {
-    L8(launch = cudaMemsetAsync(a.hist, 0, hist_bytes, st));
-    L8((bai_hist_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.sl)));
-    L8((bai_scan_kernel<<<1, kBaCta, 0, st>>>(a, n_free, a.list_off)));
-    L8((bai_scatter_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.sl, a.pos_of, a.ctrk)));
+    ADJ_LAUNCH(launch = cudaMemsetAsync(a.hist, 0, hist_bytes, st));
+    ADJ_LAUNCH((bai_hist_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.sl)));
+    ADJ_LAUNCH((bai_scan_kernel<<<1, kBaCta, 0, st>>>(a, n_free, a.list_off)));
+    ADJ_LAUNCH((bai_scatter_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.sl, a.pos_of, a.ctrk)));
   }
   if (ngf > 0 && obs > 0) {
-    L8(launch = cudaMemsetAsync(a.hist, 0, hist_bytes, st));
-    L8((bai_hist_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.gsl)));
-    L8((bai_scan_kernel<<<1, kBaCta, 0, st>>>(a, ngf, a.glist_off)));
-    L8((bai_scatter_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.gsl, a.gpos_of, a.gtrk)));
-    L8((bai_chunks_kernel<<<obs_grid, kBaiCamThreads, 0, st>>>(a)));
+    ADJ_LAUNCH(launch = cudaMemsetAsync(a.hist, 0, hist_bytes, st));
+    ADJ_LAUNCH((bai_hist_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.gsl)));
+    ADJ_LAUNCH((bai_scan_kernel<<<1, kBaCta, 0, st>>>(a, ngf, a.glist_off)));
+    ADJ_LAUNCH((bai_scatter_kernel<<<range_grid, kBaiThreads, 0, st>>>(a, a.gsl, a.gpos_of, a.gtrk)));
+    ADJ_LAUNCH((bai_chunks_kernel<<<obs_grid, kBaiCamThreads, 0, st>>>(a)));
   }
-  L8((bai_init_kernel<<<1, kBaCta, 0, st>>>(a)));
+  ADJ_LAUNCH((bai_init_kernel<<<1, kBaCta, 0, st>>>(a)));
   for (int it = 0; it < max_iters && launch == cudaSuccess; ++it) {
-    L8((bai_linearise_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
-    L8((bai_points_kernel<<<blocks(nt, kBaiThreads), kBaiThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((bai_linearise_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((bai_points_kernel<<<blocks(nt, kBaiThreads), kBaiThreads, 0, st>>>(a)));
     if (n_free > 0 || ngf > 0) {
-      if (n_free > 0) L8((bai_precond_kernel<<<blocks(nf, kBaiWarps), kBaiThreads, 0, st>>>(a)));
+      if (n_free > 0) ADJ_LAUNCH((bai_precond_kernel<<<blocks(nf, kBaiWarps), kBaiThreads, 0, st>>>(a)));
       if (ngf > 0) {
-        L8((bai_gchunk_kernel<<<blocks(nch, kBaiWarps), kBaiThreads, 0, st>>>(a)));
-        L8((bai_group_kernel<<<blocks(nq, kBaiWarps), kBaiThreads, 0, st>>>(a)));
+        ADJ_LAUNCH((bai_gchunk_kernel<<<blocks(nch, kBaiWarps), kBaiThreads, 0, st>>>(a)));
+        ADJ_LAUNCH((bai_group_kernel<<<blocks(nq, kBaiWarps), kBaiThreads, 0, st>>>(a)));
       }
-      L8(launch = cudaLaunchCooperativeKernel((const void*)bai_solve_kernel, per_sm * sms, kBaiSolveThreads,
-                                              solve_args, 0, st));
+      ADJ_LAUNCH(launch = cudaLaunchCooperativeKernel((const void*)bai_solve_kernel, per_sm * sms, kBaiSolveThreads,
+                                                      solve_args, 0, st));
     }
-    L8((bai_backsub_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
-    L8((bai_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((bai_backsub_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((bai_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
   }
-  if (obs > 0) L8(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
-  L8((bai_finish_cameras_kernel<<<cam_grid, kBaiCamThreads, 0, st>>>(a)));
-  L8((bai_finish_tracks_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
-#undef L8
+  if (obs > 0) ADJ_LAUNCH(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
+  ADJ_LAUNCH((bai_finish_cameras_kernel<<<cam_grid, kBaiCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((bai_finish_tracks_kernel<<<trk_grid, kBaiThreads, 0, st>>>(a)));
   CU(cudaFreeAsync(ws, st));
   CU(launch);
   return 0;

@@ -10,9 +10,9 @@
 //   pcg_mark_kernel      one warp per track: ba_mark_track (bundle_adjust_device.h);
 //   pcg_slot_obs_kernel  the free slot of each used observation (-1: none);
 //   pcg_hist_kernel,     the camera-major list of the used observations of the free cameras, ascending observation
-//   pcg_scan_kernel,     order within a camera, by a one-digit stable counting sort: one warp per range of kPcgRange
-//   pcg_scatter_kernel   observations counts its observations per slot, one CTA scans the counts slot after slot,
-//                        and each warp scatters its range in order;
+//   pcg_scan_kernel,     order within a camera, by the one-digit stable counting sort of bundle_adjust_device.h
+//   pcg_scatter_kernel   (ba_sort_*): one warp per range of kPcgRange observations counts its observations per slot,
+//                        one CTA scans the counts slot after slot, and each warp scatters its range in order;
 //   pcg_init_kernel      one CTA: cost0, n_used, the scale gauge's axis, the LM state (ba_init_state).
 // Per trial step (the host launches max_iters steps; each kernel returns at once when the state says the call stopped):
 //   pcg_linearise_kernel one warp per track, after an accepted step: V_p and g_p per track; W = w J_cam^T J_X per
@@ -30,9 +30,8 @@
 //   A  one thread per track: p_s = z_s + beta p'_s gathered by camera, y_p = V*_p^-1 sum W_i^T p_s(i);
 //   B  one warp per free slot: q_a = U*_a p_a - sum W_i y_p(i) over the slot's camera-major list; p_a stored; p_a . q_a;
 //   C  one thread per free slot: x += alpha p, r -= alpha q, z = M^-1 r; r . r and r . z.
-// The dot products are sums of per-slot terms; every CTA sums them itself in one fixed order (thread t takes slots
-// t, t + kPcgThreads, ..., then a fixed tree), so alpha and beta are the same in every CTA and do not depend on the
-// grid.  No floating-point atomics anywhere: a rerun gives the same bytes.
+// The loop itself, the dot products' fixed-order CTA sums and the record helpers are pcg_run and its helpers in
+// pcg_device.h.  No floating-point atomics anywhere: a rerun gives the same bytes.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -48,6 +47,8 @@
 #include "bundle_adjust.h"
 #include "device_util.h"
 #include "bundle_adjust_device.h"
+#include "pcg_device.h"
+#include "adjust_host.h"
 
 namespace cg = cooperative_groups;
 
@@ -64,11 +65,8 @@ constexpr int kPcgRange = 4096;                   // observations per warp of th
 constexpr int kPcgW = 18;                         // W [6][3] per observation
 
 // One free slot's record: U (upper by rows, 21), g_c (6), the preconditioner's Cholesky factor L (lower by rows, 21),
-// b, x, r, z (6 each), p in two buffers (12), q (6)
-constexpr int kPcU = 0, kPcG = 21, kPcL = 27, kPcB = 48, kPcX = 54, kPcR = 60, kPcZ = 66, kPcP = 72, kPcQ = 84,
-              kPcStride = 90;
-// The per-slot terms of the dot products, kPcParts arrays of n_free
-constexpr int kPartPQ = 0, kPartRR = 1, kPartRZ = 2, kPartBB = 3, kPcParts = 4;
+// then its PCG vectors (pcg_device.h): b, x, r, z (6 each), p in two buffers (12), q (6)
+constexpr int kPcU = 0, kPcG = 21, kPcL = 27, kPcB = 48, kPcX = 54, kPcP = 72, kPcQ = 84, kPcStride = 90;
 
 struct PcgArgs {
   const int* cams; const double* pts;                      // [obs], [obs][2]
@@ -89,7 +87,7 @@ struct PcgArgs {
   double* Wc;        // [18][obs]: the same, camera-major (the first list_off[n_free] columns)
   double* Jr;        // [15][obs]: J_cam, r, w, camera-major
   double* slot;      // [n_free][kPcStride]
-  double* part;      // [kPcParts][n_free]
+  double* part;      // [kPcgParts][n_free]
   BaState* state;
   int* cg_iters;     // [1]
   int* slot_of;      // [n_cams]
@@ -146,70 +144,22 @@ __global__ void __launch_bounds__(kPcgCamThreads) pcg_slot_obs_kernel(PcgArgs a)
   if (r < a.obs) a.sl[r] = a.used[r] ? a.slot_of[a.cams[r]] : -1;
 }
 
-// Warp w owns observations [w kPcgRange, (w + 1) kPcgRange) and column w of hist, so its updates need no atomics
+// The camera-major list by ba_sort_* (bundle_adjust_device.h), keyed by the free slot
 __global__ void __launch_bounds__(kPcgThreads) pcg_hist_kernel(PcgArgs a) {
-  const int lane = threadIdx.x & 31;
   const int w = blockIdx.x * kPcgWarps + (threadIdx.x >> 5);
   if (w >= a.n_ranges) return;                       // (warp-uniform)
-  const int r0 = w * kPcgRange, r1 = min(r0 + kPcgRange, a.obs);
-  for (int c0 = r0; c0 < r1; c0 += 32) {
-    const int r = c0 + lane;
-    const int s = r < r1 ? a.sl[r] : -1;
-    const unsigned peers = __match_any_sync(kFull, s);
-    if (s >= 0 && lane == __ffs(peers) - 1) a.hist[(size_t)s * a.n_ranges + w] += __popc(peers);
-    __syncwarp();
-  }
+  ba_sort_count(a.sl, a.obs, kPcgRange, a.hist, a.n_ranges, w, threadIdx.x & 31);
 }
 
-// One CTA: the exclusive prefix sum of hist in slot-major order, in place; list_off[s] = the start of slot s
 __global__ void __launch_bounds__(kBaCta) pcg_scan_kernel(PcgArgs a) {
   __shared__ int sh[kBaCta];
-  const size_t n = (size_t)a.n_free * a.n_ranges;
-  const size_t per = (n + kBaCta - 1) / kBaCta;
-  const size_t b = per * threadIdx.x, e = min(b + per, n);
-  int sum = 0;
-  for (size_t i = b; i < e; ++i) sum += a.hist[i];
-  sh[threadIdx.x] = sum;
-  __syncthreads();
-  if (threadIdx.x == 0) {                            // 1024 partial sums, scanned in order by one thread
-    int run = 0;
-    for (int q = 0; q < kBaCta; ++q) {
-      const int v = sh[q];
-      sh[q] = run;
-      run += v;
-    }
-    a.list_off[a.n_free] = run;
-  }
-  __syncthreads();
-  int run = sh[threadIdx.x];
-  for (size_t i = b; i < e; ++i) {
-    const int v = a.hist[i];
-    a.hist[i] = run;
-    if (i % a.n_ranges == 0) a.list_off[i / a.n_ranges] = run;
-    run += v;
-  }
+  ba_sort_scan(a.hist, a.n_free, a.n_ranges, a.list_off, sh);
 }
 
 __global__ void __launch_bounds__(kPcgThreads) pcg_scatter_kernel(PcgArgs a) {
-  const int lane = threadIdx.x & 31;
   const int w = blockIdx.x * kPcgWarps + (threadIdx.x >> 5);
   if (w >= a.n_ranges) return;                       // (warp-uniform)
-  const int r0 = w * kPcgRange, r1 = min(r0 + kPcgRange, a.obs);
-  for (int c0 = r0; c0 < r1; c0 += 32) {
-    const int r = c0 + lane;
-    const int s = r < r1 ? a.sl[r] : -1;
-    const unsigned peers = __match_any_sync(kFull, s);
-    if (s >= 0) {
-      int* cursor = a.hist + (size_t)s * a.n_ranges + w;
-      const int base = *cursor;
-      const int pos = base + __popc(peers & ((1u << lane) - 1u));
-      a.pos_of[r] = pos;
-      a.ctrk[pos] = a.track_of[r];
-      __syncwarp(peers);                               // every peer has read the cursor before the first one moves it
-      if (lane == __ffs(peers) - 1) *cursor = base + __popc(peers);
-    }
-    __syncwarp();
-  }
+  ba_sort_scatter(a.sl, a.obs, kPcgRange, a.hist, a.n_ranges, a.track_of, a.pos_of, a.ctrk, w, threadIdx.x & 31);
 }
 
 __global__ void __launch_bounds__(kBaCta) pcg_init_kernel(PcgArgs a) {
@@ -348,178 +298,117 @@ __global__ void __launch_bounds__(kPcgThreads) pcg_precond_kernel(PcgArgs a) {
   }
   double z[6];
   dg::pr_cholesky_apply<6>(rec + kPcL, b, z);
-  double rz = 0.0, bb = 0.0;
+  pcg_start<6>(rec + kPcB, b, z, a.part, a.n_free, s);
 #pragma unroll
-  for (int k = 0; k < 6; ++k) {
-    rec[kPcB + k] = b[k];
-    rec[kPcX + k] = 0.0;
-    rec[kPcR + k] = b[k];
-    rec[kPcZ + k] = z[k];
-    rec[kPcP + k] = 0.0;
-    rec[kPcP + 6 + k] = 0.0;
-    rec[kPcG + k] = gc[k];
-    rz += b[k] * z[k];
-    bb += b[k] * b[k];
-  }
+  for (int k = 0; k < 6; ++k) rec[kPcG + k] = gc[k];
 #pragma unroll
   for (int q = 0; q < 21; ++q) rec[kPcU + q] = active ? U[q] : 0.0;
-  a.part[kPartRZ * (size_t)a.n_free + s] = rz;
-  a.part[kPartBB * (size_t)a.n_free + s] = bb;
 }
 
-// The fixed-order sums over the free slots of up to two per-slot arrays, the same in every CTA: thread t adds slots
-// t, t + kPcgSolveThreads, ... in turn, then a tree over the threads.  Every thread gets the sums.
-__device__ void cta_sum2(const double* u, const double* v, int n, double* sh, double* su, double* sv) {
-  double x = 0.0, y = 0.0;
-  for (int i = threadIdx.x; i < n; i += kPcgSolveThreads) {
-    x += __ldcg(u + i);
-    if (v) y += __ldcg(v + i);
-  }
-  sh[threadIdx.x] = x;
-  sh[kPcgSolveThreads + threadIdx.x] = y;
-  __syncthreads();
-  for (int s = kPcgSolveThreads / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) {
-      sh[threadIdx.x] += sh[threadIdx.x + s];
-      sh[kPcgSolveThreads + threadIdx.x] += sh[kPcgSolveThreads + threadIdx.x + s];
-    }
-    __syncthreads();
-  }
-  *su = sh[0];
-  *sv = sh[kPcgSolveThreads];
-  __syncthreads();
-}
+// pcg_run's S p and phase C over the free slots.  product: A, one thread per track, y_p = V*_p^-1 sum W_i^T p_s(i);
+// grid.sync; B, one warp per free slot, q_a = U*_a p_a - sum W_i y_p(i), p_a stored, p_a . q_a.  update: one thread
+// per free slot.
+struct PcgSchur {
+  const PcgArgs& a;
+  int tid, nthr, lane, warp, nwarps;
+  double lam;
+  int hold_row;
 
-// p_s = z_s + beta p'_s of slot s, p' in buffer `prev`
-__device__ __forceinline__ void direction(const PcgArgs& a, int s, int prev, double beta, double* p) {
-  const double* rec = slot_rec(a, s);
+  __device__ __forceinline__ void product(cg::grid_group& grid, int cur, int prev, double beta) const {
+    const int nf = a.n_free;
+    const size_t no = (size_t)a.obs;
+    for (int j = tid; j < a.n_tracks; j += nthr) {
+      if (a.trk_used[j] == 0) continue;
+      const int b = a.offsets[j], e = a.offsets[j + 1];
+      double u[3] = {0.0, 0.0, 0.0};
+      for (int r = b; r < e; ++r) {
+        const int s = a.sl[r];
+        if (s < 0) continue;
+        double p[6];
+        pcg_direction<6>(slot_rec(a, s) + kPcB, prev, beta, p);
 #pragma unroll
-  for (int k = 0; k < 6; ++k) p[k] = __ldcg(rec + kPcZ + k) + beta * __ldcg(rec + kPcP + 6 * prev + k);
-}
+        for (int k = 0; k < 6; ++k)
+#pragma unroll
+          for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wt + (3 * k + m) * no + r) * p[k];
+      }
+      double yv[3];
+      dg::ba_sym3_mul(a.trk + dg::kBaTrkStride * (size_t)j + dg::kBaTrkVi, u, yv);
+#pragma unroll
+      for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
+    }
+    grid.sync();
+    for (int s = warp; s < nf; s += nwarps) {
+      double acc[6] = {0, 0, 0, 0, 0, 0};
+      const int i0 = a.list_off[s], i1 = a.list_off[s + 1];
+      for (int i = i0 + lane; i < i1; i += 32) {
+        const double* yp = a.y + 3 * (size_t)a.ctrk[i];
+        const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
+#pragma unroll
+        for (int k = 0; k < 6; ++k)
+          acc[k] += __ldg(a.Wc + (3 * k) * no + i) * y0 + __ldg(a.Wc + (3 * k + 1) * no + i) * y1 +
+                    __ldg(a.Wc + (3 * k + 2) * no + i) * y2;
+      }
+#pragma unroll
+      for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
+      if (lane == 0) {
+        double p[6];
+        double* rec = slot_rec(a, s);
+        pcg_direction<6>(rec + kPcB, prev, beta, p);
+        const double* U = rec + kPcU;
+        const int hold = hold_row - dg::kBaCamParams * s;
+        double pq = 0.0;
+#pragma unroll
+        for (int k = 0; k < 6; ++k) {
+          double v = -acc[k];
+#pragma unroll
+          for (int l = 0; l < 6; ++l) {
+            const int m = k <= l ? k * 6 - k * (k - 1) / 2 + (l - k) : l * 6 - l * (l - 1) / 2 + (k - l);
+            v += U[m] * p[l];
+          }
+          const int d = k * 6 - k * (k - 1) / 2;
+          v += lam * U[d] * p[k];
+          if (k == hold) v = p[k];
+          rec[kPcQ + k] = v;
+          rec[kPcP + 6 * cur + k] = p[k];
+          pq += p[k] * v;
+        }
+        a.part[kPartPQ * (size_t)nf + s] = pq;
+      }
+    }
+  }
 
-// The PCG loop of one trial step, then the trial poses of the free cameras.  Data written inside the launch is read
-// with __ldcg (L2), as other CTAs wrote it; every CTA computes the same scalars, so every CTA takes the same branches
-// and meets the same grid.sync() calls.
+  __device__ __forceinline__ void update(int cur, int /*prev*/, double /*beta*/, double alpha) const {
+    const int nf = a.n_free;
+    for (int s = tid; s < nf; s += nthr) {
+      double* rec = slot_rec(a, s);
+      double p[6], q[6];
+#pragma unroll
+      for (int k = 0; k < 6; ++k) {
+        p[k] = __ldcg(rec + kPcP + 6 * cur + k);
+        q[k] = __ldcg(rec + kPcQ + k);
+      }
+      const double2 rz = pcg_update<6>(rec + kPcB, p, q, alpha, [rec](const double* r, double* z) {
+        dg::pr_cholesky_apply<6>(rec + kPcL, r, z);
+      });
+      a.part[kPartRR * (size_t)nf + s] = rz.x;
+      a.part[kPartRZ * (size_t)nf + s] = rz.y;
+    }
+  }
+};
+
+// The PCG loop of one trial step (pcg_run), then the trial poses of the free cameras
 __global__ void __launch_bounds__(kPcgSolveThreads) pcg_solve_kernel(PcgArgs a) {
   __shared__ double sh[2 * kPcgSolveThreads];
   BaState* st = a.state;
   if (st->stop || st->bad) return;                     // (grid-uniform: nothing below writes them before a grid.sync)
   cg::grid_group grid = cg::this_grid();
   const int tid = blockIdx.x * kPcgSolveThreads + threadIdx.x, nthr = gridDim.x * kPcgSolveThreads;
-  const int lane = threadIdx.x & 31, warp = tid >> 5, nwarps = nthr >> 5;
   const int nf = a.n_free;
-  const size_t no = (size_t)a.obs;
-  const double lam = st->lam;
-  const int hold_row = st->hold_row;
-  double bb, rho;
-  cta_sum2(a.part + kPartBB * (size_t)nf, a.part + kPartRZ * (size_t)nf, nf, sh, &bb, &rho);
-  int it = 0;
-  bool reject = false;
-  if (bb > 0.0) {
-    double beta = 0.0;
-    for (;;) {
-      const int cur = it & 1, prev = cur ^ 1;
-      // A: y_p = V*_p^-1 sum W_i^T p_s(i)
-      for (int j = tid; j < a.n_tracks; j += nthr) {
-        if (a.trk_used[j] == 0) continue;
-        const int b = a.offsets[j], e = a.offsets[j + 1];
-        double u[3] = {0.0, 0.0, 0.0};
-        for (int r = b; r < e; ++r) {
-          const int s = a.sl[r];
-          if (s < 0) continue;
-          double p[6];
-          direction(a, s, prev, beta, p);
-#pragma unroll
-          for (int k = 0; k < 6; ++k)
-#pragma unroll
-            for (int m = 0; m < 3; ++m) u[m] += __ldg(a.Wt + (3 * k + m) * no + r) * p[k];
-        }
-        double yv[3];
-        dg::ba_sym3_mul(a.trk + dg::kBaTrkStride * (size_t)j + dg::kBaTrkVi, u, yv);
-#pragma unroll
-        for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
-      }
-      grid.sync();
-      // B: q_a = U*_a p_a - sum W_i y_p(i)
-      for (int s = warp; s < nf; s += nwarps) {
-        double acc[6] = {0, 0, 0, 0, 0, 0};
-        const int i0 = a.list_off[s], i1 = a.list_off[s + 1];
-        for (int i = i0 + lane; i < i1; i += 32) {
-          const double* yp = a.y + 3 * (size_t)a.ctrk[i];
-          const double y0 = __ldcg(yp), y1 = __ldcg(yp + 1), y2 = __ldcg(yp + 2);
-#pragma unroll
-          for (int k = 0; k < 6; ++k)
-            acc[k] += __ldg(a.Wc + (3 * k) * no + i) * y0 + __ldg(a.Wc + (3 * k + 1) * no + i) * y1 +
-                      __ldg(a.Wc + (3 * k + 2) * no + i) * y2;
-        }
-#pragma unroll
-        for (int k = 0; k < 6; ++k) acc[k] = warp_sum(acc[k]);
-        if (lane == 0) {
-          double p[6];
-          direction(a, s, prev, beta, p);
-          double* rec = slot_rec(a, s);
-          const double* U = rec + kPcU;
-          const int hold = hold_row - dg::kBaCamParams * s;
-          double pq = 0.0;
-#pragma unroll
-          for (int k = 0; k < 6; ++k) {
-            double v = -acc[k];
-#pragma unroll
-            for (int l = 0; l < 6; ++l) {
-              const int m = k <= l ? k * 6 - k * (k - 1) / 2 + (l - k) : l * 6 - l * (l - 1) / 2 + (k - l);
-              v += U[m] * p[l];
-            }
-            const int d = k * 6 - k * (k - 1) / 2;
-            v += lam * U[d] * p[k];
-            if (k == hold) v = p[k];
-            rec[kPcQ + k] = v;
-            rec[kPcP + 6 * cur + k] = p[k];
-            pq += p[k] * v;
-          }
-          a.part[kPartPQ * (size_t)nf + s] = pq;
-        }
-      }
-      grid.sync();
-      // C: alpha, x, r, z
-      double kappa, unused;
-      cta_sum2(a.part + kPartPQ * (size_t)nf, nullptr, nf, sh, &kappa, &unused);
-      ++it;
-      if (!(kappa > 0.0) || !finite(kappa)) {
-        reject = it == 1;
-        break;
-      }
-      const double alpha = rho / kappa;
-      for (int s = tid; s < nf; s += nthr) {
-        double* rec = slot_rec(a, s);
-        double r[6], z[6];
-        double rr = 0.0, rz = 0.0;
-#pragma unroll
-        for (int k = 0; k < 6; ++k) {
-          rec[kPcX + k] = __ldcg(rec + kPcX + k) + alpha * __ldcg(rec + kPcP + 6 * cur + k);
-          r[k] = __ldcg(rec + kPcR + k) - alpha * __ldcg(rec + kPcQ + k);
-        }
-        dg::pr_cholesky_apply<6>(rec + kPcL, r, z);
-#pragma unroll
-        for (int k = 0; k < 6; ++k) {
-          rec[kPcR + k] = r[k];
-          rec[kPcZ + k] = z[k];
-          rr += r[k] * r[k];
-          rz += r[k] * z[k];
-        }
-        a.part[kPartRR * (size_t)nf + s] = rr;
-        a.part[kPartRZ * (size_t)nf + s] = rz;
-      }
-      grid.sync();
-      double rr, rz;
-      cta_sum2(a.part + kPartRR * (size_t)nf, a.part + kPartRZ * (size_t)nf, nf, sh, &rr, &rz);
-      if (rr <= a.cg_tol2 * bb || it >= a.cg_max_iters) break;
-      beta = rz / rho;
-      rho = rz;
-    }
-  }
+  const PcgSchur op{a, tid, nthr, (int)threadIdx.x & 31, tid >> 5, nthr >> 5, st->lam, st->hold_row};
+  const PcgResult res = pcg_run<kPcgSolveThreads>(grid, a.part, nf, a.cg_tol2, a.cg_max_iters, sh, op);
   // the trial poses (x of a slot was last written by this thread, in phase C)
   const int cur = st->cur;
-  if (!reject)
+  if (!res.reject)
     for (int s = tid; s < nf; s += nthr) {
       if (!slot_active(a, s)) continue;
       const int c = a.free[s];
@@ -530,8 +419,8 @@ __global__ void __launch_bounds__(kPcgSolveThreads) pcg_solve_kernel(PcgArgs a) 
       for (int i = 0; i < 12; ++i) out[i] = P2[i];
     }
   if (tid == 0) {
-    a.cg_iters[0] += it;
-    if (reject) st->bad = 1;
+    a.cg_iters[0] += res.iters;
+    if (res.reject) st->bad = 1;
   }
 }
 
@@ -595,15 +484,6 @@ __global__ void __launch_bounds__(kPcgThreads) pcg_finish_tracks_kernel(PcgArgs 
   ba_finish_track(a, j, lane);
 }
 
-template <typename T>
-T* carve(char*& p, size_t count) {
-  T* out = (T*)p;
-  p += (sizeof(T) * count + 255) / 256 * 256;
-  return out;
-}
-
-int blocks(size_t n, int per) { return (int)((n + per - 1) / per); }
-
 }  // namespace
 
 extern "C" {
@@ -629,56 +509,51 @@ int dgb200_bundle_adjust_pcg_ragged_dev(const int32_t* d_cams, const double* d_p
   if (cg_max_iters < 1) return fail(DGB200_E_ARG, "cg_max_iters must be at least 1");
   if (!(cg_tol >= 0.0) || !(cg_tol < INFINITY)) return fail(DGB200_E_ARG, "cg_tol must be a non-negative finite number");
   const cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  CU(cudaGetDevice(&dev));
-  CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) return fail(DGB200_E_CUDA, "the device does not support cooperative launches");
+  int sms = 0, per_sm = 0;
+  cudaError_t e = cudaSuccess;
+  if (const char* m = coop_sms(&sms, &e)) return fail(DGB200_E_CUDA, m, e);
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, pcg_solve_kernel, kPcgSolveThreads, 0));
   if (per_sm < 1) return fail(DGB200_E_CUDA, "pcg_solve_kernel does not fit on an SM");
   const int n_ranges = obs > 0 ? blocks((size_t)obs, kPcgRange) : 1;
   const size_t no = (size_t)(obs > 0 ? obs : 1), nt = (size_t)n_tracks, nc = (size_t)n_cams;
   const size_t nf = (size_t)(n_free > 0 ? n_free : 1);
-  size_t bytes = 0;
-  {                                                    // the carve below, counted
-    const size_t d = sizeof(double), i = sizeof(int);
-    const size_t sizes[] = {d * dg::kTrCamStride * nc, d * 24 * nc, d * 6 * nt, d * dg::kBaTrkStride * nt, d * 3 * nt,
-                            d * kPcgW * no, d * kPcgW * no, d * 15 * no, d * kPcStride * nf, d * kPcParts * nf,
-                            sizeof(BaState), i, i * nf, i * nc, i * no, i * no, i * no, i * no,
-                            i * nf * (size_t)n_ranges, i * (nf + 1), i * nt, no, no};
-    for (size_t s : sizes) bytes += (s + 255) / 256 * 256;
-  }
-  char* ws = nullptr;
-  CU(cudaMallocAsync((void**)&ws, bytes, st));
   PcgArgs a;
   a.cams = d_cams; a.pts = d_pts; a.R = d_R; a.t = d_t; a.K = d_K; a.k_per_camera = k_per_camera; a.n_cams = n_cams;
   a.offsets = d_offsets; a.mask = d_mask; a.X = d_X; a.n_tracks = n_tracks; a.obs = obs; a.n_free = n_free;
   a.gauge_slot = gauge_slot; a.held_cam = held_cam; a.n_ranges = n_ranges; a.cg_max_iters = cg_max_iters;
   a.sig2 = loss_scale * loss_scale; a.th2 = px_th * px_th; a.cg_tol2 = cg_tol * cg_tol;
-  char* p = ws;
-  a.tab = carve<double>(p, dg::kTrCamStride * nc);
-  a.poses = carve<double>(p, 24 * nc);
-  a.Xb = carve<double>(p, 6 * nt);
-  a.trk = carve<double>(p, dg::kBaTrkStride * nt);
-  a.y = carve<double>(p, 3 * nt);
-  a.Wt = carve<double>(p, kPcgW * no);
-  a.Wc = carve<double>(p, kPcgW * no);
-  a.Jr = carve<double>(p, 15 * no);
-  a.slot = carve<double>(p, kPcStride * nf);
-  a.part = carve<double>(p, kPcParts * nf);
-  a.state = carve<BaState>(p, 1);
-  a.cg_iters = carve<int>(p, 1);
-  int* d_free = carve<int>(p, nf);
-  a.slot_of = carve<int>(p, nc);
-  a.track_of = carve<int>(p, no);
-  a.sl = carve<int>(p, no);
-  a.pos_of = carve<int>(p, no);
-  a.ctrk = carve<int>(p, no);
-  a.hist = carve<int>(p, nf * (size_t)n_ranges);
-  a.list_off = carve<int>(p, nf + 1);
-  a.trk_used = carve<int>(p, nt);
-  a.usable = carve<unsigned char>(p, no);
-  a.used = carve<unsigned char>(p, no);
+  int* d_free = nullptr;
+  auto lay_out = [&](char* base) {
+    Carve w{base};
+    a.tab = w.take<double>(dg::kTrCamStride * nc);
+    a.poses = w.take<double>(24 * nc);
+    a.Xb = w.take<double>(6 * nt);
+    a.trk = w.take<double>(dg::kBaTrkStride * nt);
+    a.y = w.take<double>(3 * nt);
+    a.Wt = w.take<double>(kPcgW * no);
+    a.Wc = w.take<double>(kPcgW * no);
+    a.Jr = w.take<double>(15 * no);
+    a.slot = w.take<double>(kPcStride * nf);
+    a.part = w.take<double>(kPcgParts * nf);
+    a.state = w.take<BaState>(1);
+    a.cg_iters = w.take<int>(1);
+    d_free = w.take<int>(nf);
+    a.slot_of = w.take<int>(nc);
+    a.track_of = w.take<int>(no);
+    a.sl = w.take<int>(no);
+    a.pos_of = w.take<int>(no);
+    a.ctrk = w.take<int>(no);
+    a.hist = w.take<int>(nf * (size_t)n_ranges);
+    a.list_off = w.take<int>(nf + 1);
+    a.trk_used = w.take<int>(nt);
+    a.usable = w.take<unsigned char>(no);
+    a.used = w.take<unsigned char>(no);
+    return w.bytes;
+  };
+  char* ws = nullptr;
+  const size_t bytes = lay_out(nullptr);
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
+  lay_out(ws);
   a.free = d_free;
   a.R_out = d_R_out; a.t_out = d_t_out; a.X_out = d_X_out; a.mask_out = d_mask_out;
   a.cost0_out = d_cost0_out; a.cost_out = d_cost_out; a.iters_out = d_iters_out; a.n_used_out = d_n_used_out;
@@ -690,42 +565,37 @@ int dgb200_bundle_adjust_pcg_ragged_dev(const int32_t* d_cams, const double* d_p
   const int slot_grid = blocks(nf, kPcgWarps);
   void* solve_args[] = {&a};
   cudaError_t launch = cudaSuccess;
-#define L6(...)                                   \
-  if (launch == cudaSuccess) {                    \
-    __VA_ARGS__;                                  \
-    launch = cudaGetLastError();                  \
-  }
-  if (n_free > 0) L6(launch = cudaMemcpyAsync(d_free, h_free, sizeof(int) * (size_t)n_free, cudaMemcpyHostToDevice, st));
-  L6(launch = cudaMemsetAsync(a.usable, 0, no, st));       // rows outside every span are neither usable nor used
-  L6(launch = cudaMemsetAsync(a.used, 0, no, st));
-  L6(launch = cudaMemsetAsync(a.slot_of, 0xff, sizeof(int) * nc, st));
-  L6(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nf + 1), st));
-  L6(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nf * (size_t)n_ranges, st));
-  L6((pcg_cameras_kernel<<<cam_grid, kPcgCamThreads, 0, st>>>(a)));
-  if (n_free > 0) L6((pcg_slots_kernel<<<blocks(nf, kPcgCamThreads), kPcgCamThreads, 0, st>>>(a)));
-  L6((pcg_mark_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
-  if (obs > 0) L6((pcg_slot_obs_kernel<<<obs_grid, kPcgCamThreads, 0, st>>>(a)));
+  if (n_free > 0)
+    ADJ_LAUNCH(launch = cudaMemcpyAsync(d_free, h_free, sizeof(int) * (size_t)n_free, cudaMemcpyHostToDevice, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.usable, 0, no, st));   // rows outside every span are neither usable nor used
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.used, 0, no, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.slot_of, 0xff, sizeof(int) * nc, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nf + 1), st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nf * (size_t)n_ranges, st));
+  ADJ_LAUNCH((pcg_cameras_kernel<<<cam_grid, kPcgCamThreads, 0, st>>>(a)));
+  if (n_free > 0) ADJ_LAUNCH((pcg_slots_kernel<<<blocks(nf, kPcgCamThreads), kPcgCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((pcg_mark_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
+  if (obs > 0) ADJ_LAUNCH((pcg_slot_obs_kernel<<<obs_grid, kPcgCamThreads, 0, st>>>(a)));
   if (n_free > 0 && obs > 0) {
-    L6((pcg_hist_kernel<<<range_grid, kPcgThreads, 0, st>>>(a)));
-    L6((pcg_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
-    L6((pcg_scatter_kernel<<<range_grid, kPcgThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_hist_kernel<<<range_grid, kPcgThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_scatter_kernel<<<range_grid, kPcgThreads, 0, st>>>(a)));
   }
-  L6((pcg_init_kernel<<<1, kBaCta, 0, st>>>(a)));
+  ADJ_LAUNCH((pcg_init_kernel<<<1, kBaCta, 0, st>>>(a)));
   for (int it = 0; it < max_iters && launch == cudaSuccess; ++it) {
-    L6((pcg_linearise_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
-    L6((pcg_points_kernel<<<blocks(nt, kPcgThreads), kPcgThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_linearise_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_points_kernel<<<blocks(nt, kPcgThreads), kPcgThreads, 0, st>>>(a)));
     if (n_free > 0) {
-      L6((pcg_precond_kernel<<<slot_grid, kPcgThreads, 0, st>>>(a)));
-      L6(launch = cudaLaunchCooperativeKernel((const void*)pcg_solve_kernel, per_sm * sms, kPcgSolveThreads,
-                                              solve_args, 0, st));
+      ADJ_LAUNCH((pcg_precond_kernel<<<slot_grid, kPcgThreads, 0, st>>>(a)));
+      ADJ_LAUNCH(launch = cudaLaunchCooperativeKernel((const void*)pcg_solve_kernel, per_sm * sms, kPcgSolveThreads,
+                                                      solve_args, 0, st));
     }
-    L6((pcg_backsub_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
-    L6((pcg_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_backsub_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((pcg_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
   }
-  if (obs > 0) L6(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
-  L6((pcg_finish_cameras_kernel<<<cam_grid, kPcgCamThreads, 0, st>>>(a)));
-  L6((pcg_finish_tracks_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
-#undef L6
+  if (obs > 0) ADJ_LAUNCH(launch = cudaMemsetAsync(d_mask_out, 0, (size_t)obs, st));   // rows outside every span
+  ADJ_LAUNCH((pcg_finish_cameras_kernel<<<cam_grid, kPcgCamThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((pcg_finish_tracks_kernel<<<trk_grid, kPcgThreads, 0, st>>>(a)));
   CU(cudaFreeAsync(ws, st));
   CU(launch);
   return 0;

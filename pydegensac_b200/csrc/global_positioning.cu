@@ -32,8 +32,8 @@
 //
 // One PCG iteration: A, one thread per track: y_j = V*_j^-1 sum m_o p_i(o); B, one warp per view: q_i = U*_i p_i -
 // sum m_o y_j(o) over its camera-major list, p_i . q_i; C, one thread per view: x += alpha p, r -= alpha q, z = M^-1 r;
-// r . r and r . z.  The dot products are sums of per-view terms that every CTA sums itself in one fixed order, so they
-// do not depend on the grid.  No floating-point atomics anywhere: a rerun gives the same bytes.
+// r . r and r . z; the loop is pcg_run (pcg_device.h), whose dot products every CTA sums itself in one fixed order, so
+// they do not depend on the grid.  No floating-point atomics anywhere: a rerun gives the same bytes.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -47,6 +47,8 @@
 #include "tracks.h"
 #include "device_util.h"
 #include "bundle_adjust_device.h"
+#include "pcg_device.h"
+#include "adjust_host.h"
 
 namespace cg = cooperative_groups;
 
@@ -70,10 +72,9 @@ constexpr int kGtQ = 0, kGtH = 6, kGtUH = 9, kGtS = 12;
 static_assert(dg::kBaTrkCost == 15 && dg::kBaTrkStride == 16, "the track record shares bundle_adjust.h's cost slot");
 // One track's V*^-1 (upper, 6) and t = V*^-1 g (3)
 constexpr int kGvVi = 0, kGvT = 6, kGvStride = 9;
-// One view's record: U* (upper, 6), the preconditioner's Cholesky factor L (lower, 6), b, x, r, z (3 each), p in two
-// buffers (6), q (3)
-constexpr int kGcU = 0, kGcL = 6, kGcB = 12, kGcX = 15, kGcR = 18, kGcZ = 21, kGcP = 24, kGcQ = 30, kGcStride = 33;
-constexpr int kPartPQ = 0, kPartRR = 1, kPartRZ = 2, kPartBB = 3, kGpParts = 4;
+// One view's record: U* (upper, 6), the preconditioner's Cholesky factor L (lower, 6), then its PCG vectors
+// (pcg_device.h): b, x, r, z (3 each), p in two buffers (6), q (3)
+constexpr int kGcU = 0, kGcL = 6, kGcB = 12, kGcX = 15, kGcP = 24, kGcQ = 30, kGcStride = 33;
 
 struct GpArgs {
   const int* cams; const double* pts;                      // [obs], [obs][2]
@@ -95,7 +96,7 @@ struct GpArgs {
   double* tv;        // [T][kGvStride]
   double* y;         // [T][3]
   double* rec;       // [n_cams][kGcStride]
-  double* part;      // [kGpParts][n_cams]
+  double* part;      // [kPcgParts][n_cams]
   BaState* state;
   int* cg_iters;     // [1]
   int* linbad;       // [1]: the linearisation has an observation with |a| = 0 or not finite
@@ -440,168 +441,105 @@ __global__ void __launch_bounds__(32 * kGpWarps) gp_precond_kernel(GpArgs a) {
 #pragma unroll
   for (int k = 0; k < 3; ++k) b[k] = act ? bv[k] : 0.0;
   dg::pr_cholesky_apply<3>(rec + kGcL, b, z);
-  double rz = 0.0, bb = 0.0;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    rec[kGcB + k] = b[k];
-    rec[kGcX + k] = 0.0;
-    rec[kGcR + k] = b[k];
-    rec[kGcZ + k] = z[k];
-    rec[kGcP + k] = 0.0;
-    rec[kGcP + 3 + k] = 0.0;
-    rz += b[k] * z[k];
-    bb += b[k] * b[k];
-  }
+  pcg_start<3>(rec + kGcB, b, z, a.part, a.n_cams, c);
 #pragma unroll
   for (int m = 0; m < 6; ++m) rec[kGcU + m] = act ? U[m] : 0.0;
-  a.part[kPartRZ * (size_t)a.n_cams + c] = rz;
-  a.part[kPartBB * (size_t)a.n_cams + c] = bb;
 }
 
-// The fixed-order sums over the views of up to two per-view arrays, the same in every CTA: thread t adds views t,
-// t + kGpSolveThreads, ... in turn, then a tree over the threads.  Every thread gets the sums.
-__device__ void cta_sum2(const double* u, const double* v, int n, double* sh, double* su, double* sv) {
-  double x = 0.0, y = 0.0;
-  for (int i = threadIdx.x; i < n; i += kGpSolveThreads) {
-    x += __ldcg(u + i);
-    if (v) y += __ldcg(v + i);
-  }
-  sh[threadIdx.x] = x;
-  sh[kGpSolveThreads + threadIdx.x] = y;
-  __syncthreads();
-  for (int s = kGpSolveThreads / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) {
-      sh[threadIdx.x] += sh[threadIdx.x + s];
-      sh[kGpSolveThreads + threadIdx.x] += sh[kGpSolveThreads + threadIdx.x + s];
-    }
-    __syncthreads();
-  }
-  *su = sh[0];
-  *sv = sh[kGpSolveThreads];
-  __syncthreads();
-}
+// pcg_run's S p and phase C over the views.  product: A, one thread per track, y_j = V*_j^-1 sum m_o p_i(o); grid.sync;
+// B, one warp per view, q_c = U*_c p_c - sum m_o y_j(o), p_c stored, p_c . q_c.  update: one thread per view.
+struct GpSchur {
+  const GpArgs& a;
+  int tid, nthr, lane, warp, nwarps;
+  double f;
 
-// p_c = z_c + beta p'_c, p' in buffer `prev`
-__device__ __forceinline__ void direction(const GpArgs& a, int c, int prev, double beta, double* p) {
-  const double* rec = view_rec(a, c);
+  __device__ __forceinline__ void product(cg::grid_group& grid, int cur, int prev, double beta) const {
+    const int nc = a.n_cams;
+    const size_t no = (size_t)a.obs;
+    for (int j = tid; j < a.n_tracks; j += nthr) {
+      if (a.trk_used[j] == 0) continue;
+      const int b = a.offsets[j], e = a.offsets[j + 1];
+      double acc[3] = {0.0, 0.0, 0.0};
+      for (int r = b; r < e; ++r) {
+        const int k = a.key[r];
+        if (k < 0) continue;
+        double p[3], mp[3];
+        pcg_direction<3>(view_rec(a, k) + kGcB, prev, beta, p);
+        const double u[3] = {__ldg(a.lo + kLoU * no + r), __ldg(a.lo + (kLoU + 1) * no + r),
+                             __ldg(a.lo + (kLoU + 2) * no + r)};
+        dg::gp_m_apply(u, __ldg(a.lo + kLoS * no + r), f, p, mp);
+        acc[0] += mp[0]; acc[1] += mp[1]; acc[2] += mp[2];
+      }
+      double yv[3];
+      dg::ba_sym3_mul(a.tv + kGvStride * (size_t)j + kGvVi, acc, yv);
 #pragma unroll
-  for (int k = 0; k < 3; ++k) p[k] = __ldcg(rec + kGcZ + k) + beta * __ldcg(rec + kGcP + 3 * prev + k);
-}
+      for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
+    }
+    grid.sync();
+    for (int c = warp; c < nc; c += nwarps) {
+      double acc[3] = {0.0, 0.0, 0.0};
+      const int i0 = a.list_off[c], i1 = a.list_off[c + 1];
+      for (int i = i0 + lane; i < i1; i += 32) {
+        const double* yp = a.y + 3 * (size_t)a.ctrk[i];
+        const double yv[3] = {__ldcg(yp), __ldcg(yp + 1), __ldcg(yp + 2)};
+        const double u[3] = {__ldg(a.lc + kLcU * no + i), __ldg(a.lc + (kLcU + 1) * no + i),
+                             __ldg(a.lc + (kLcU + 2) * no + i)};
+        double my[3];
+        dg::gp_m_apply(u, __ldg(a.lc + kLcS * no + i), f, yv, my);
+        acc[0] += my[0]; acc[1] += my[1]; acc[2] += my[2];
+      }
+#pragma unroll
+      for (int k = 0; k < 3; ++k) acc[k] = warp_sum(acc[k]);
+      if (lane == 0) {
+        double p[3], Up[3];
+        double* rec = view_rec(a, c);
+        pcg_direction<3>(rec + kGcB, prev, beta, p);
+        dg::ba_sym3_mul(rec + kGcU, p, Up);
+        double pq = 0.0;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const double q = Up[k] - acc[k];
+          rec[kGcQ + k] = q;
+          rec[kGcP + 3 * cur + k] = p[k];
+          pq += p[k] * q;
+        }
+        a.part[kPartPQ * (size_t)nc + c] = pq;
+      }
+    }
+  }
 
-// The PCG loop of one trial step, then the trial centres.  Data written inside the launch is read with __ldcg (L2), as
-// other CTAs wrote it; every CTA computes the same scalars, so every CTA takes the same branches and meets the same
-// grid.sync() calls.
+  __device__ __forceinline__ void update(int cur, int /*prev*/, double /*beta*/, double alpha) const {
+    const int nc = a.n_cams;
+    for (int c = tid; c < nc; c += nthr) {
+      double* rec = view_rec(a, c);
+      double p[3], q[3];
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        p[k] = __ldcg(rec + kGcP + 3 * cur + k);
+        q[k] = __ldcg(rec + kGcQ + k);
+      }
+      const double2 rz = pcg_update<3>(rec + kGcB, p, q, alpha, [rec](const double* r, double* z) {
+        dg::pr_cholesky_apply<3>(rec + kGcL, r, z);
+      });
+      a.part[kPartRR * (size_t)nc + c] = rz.x;
+      a.part[kPartRZ * (size_t)nc + c] = rz.y;
+    }
+  }
+};
+
+// The PCG loop of one trial step (pcg_run), then the trial centres
 __global__ void __launch_bounds__(kGpSolveThreads) gp_solve_kernel(GpArgs a) {
   __shared__ double sh[2 * kGpSolveThreads];
   BaState* st = a.state;
   if (st->stop || st->bad) return;                   // (grid-uniform: nothing below writes them before a grid.sync)
   cg::grid_group grid = cg::this_grid();
   const int tid = blockIdx.x * kGpSolveThreads + threadIdx.x, nthr = gridDim.x * kGpSolveThreads;
-  const int lane = threadIdx.x & 31, warp = tid >> 5, nwarps = nthr >> 5;
   const int nc = a.n_cams;
-  const size_t no = (size_t)a.obs;
-  const double f = 1.0 / (1.0 + st->lam);
-  double bb, rho;
-  cta_sum2(a.part + kPartBB * (size_t)nc, a.part + kPartRZ * (size_t)nc, nc, sh, &bb, &rho);
-  int it = 0;
-  bool reject = false;
-  if (bb > 0.0) {
-    double beta = 0.0;
-    for (;;) {
-      const int cur = it & 1, prev = cur ^ 1;
-      // A: y_j = V*_j^-1 sum m_o p_i(o)
-      for (int j = tid; j < a.n_tracks; j += nthr) {
-        if (a.trk_used[j] == 0) continue;
-        const int b = a.offsets[j], e = a.offsets[j + 1];
-        double acc[3] = {0.0, 0.0, 0.0};
-        for (int r = b; r < e; ++r) {
-          const int k = a.key[r];
-          if (k < 0) continue;
-          double p[3], mp[3];
-          direction(a, k, prev, beta, p);
-          const double u[3] = {__ldg(a.lo + kLoU * no + r), __ldg(a.lo + (kLoU + 1) * no + r),
-                               __ldg(a.lo + (kLoU + 2) * no + r)};
-          dg::gp_m_apply(u, __ldg(a.lo + kLoS * no + r), f, p, mp);
-          acc[0] += mp[0]; acc[1] += mp[1]; acc[2] += mp[2];
-        }
-        double yv[3];
-        dg::ba_sym3_mul(a.tv + kGvStride * (size_t)j + kGvVi, acc, yv);
-#pragma unroll
-        for (int m = 0; m < 3; ++m) a.y[3 * (size_t)j + m] = yv[m];
-      }
-      grid.sync();
-      // B: q_c = U*_c p_c - sum m_o y_j(o)
-      for (int c = warp; c < nc; c += nwarps) {
-        double acc[3] = {0.0, 0.0, 0.0};
-        const int i0 = a.list_off[c], i1 = a.list_off[c + 1];
-        for (int i = i0 + lane; i < i1; i += 32) {
-          const double* yp = a.y + 3 * (size_t)a.ctrk[i];
-          const double yv[3] = {__ldcg(yp), __ldcg(yp + 1), __ldcg(yp + 2)};
-          const double u[3] = {__ldg(a.lc + kLcU * no + i), __ldg(a.lc + (kLcU + 1) * no + i),
-                               __ldg(a.lc + (kLcU + 2) * no + i)};
-          double my[3];
-          dg::gp_m_apply(u, __ldg(a.lc + kLcS * no + i), f, yv, my);
-          acc[0] += my[0]; acc[1] += my[1]; acc[2] += my[2];
-        }
-#pragma unroll
-        for (int k = 0; k < 3; ++k) acc[k] = warp_sum(acc[k]);
-        if (lane == 0) {
-          double p[3], Up[3];
-          direction(a, c, prev, beta, p);
-          double* rec = view_rec(a, c);
-          dg::ba_sym3_mul(rec + kGcU, p, Up);
-          double pq = 0.0;
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            const double q = Up[k] - acc[k];
-            rec[kGcQ + k] = q;
-            rec[kGcP + 3 * cur + k] = p[k];
-            pq += p[k] * q;
-          }
-          a.part[kPartPQ * (size_t)nc + c] = pq;
-        }
-      }
-      grid.sync();
-      // C: alpha, x, r, z
-      double kappa, unused;
-      cta_sum2(a.part + kPartPQ * (size_t)nc, nullptr, nc, sh, &kappa, &unused);
-      ++it;
-      if (!(kappa > 0.0) || !finite(kappa)) {
-        reject = it == 1;
-        break;
-      }
-      const double alpha = rho / kappa;
-      for (int c = tid; c < nc; c += nthr) {
-        double* rec = view_rec(a, c);
-        double r[3], z[3];
-        double rr = 0.0, rz = 0.0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          rec[kGcX + k] = __ldcg(rec + kGcX + k) + alpha * __ldcg(rec + kGcP + 3 * cur + k);
-          r[k] = __ldcg(rec + kGcR + k) - alpha * __ldcg(rec + kGcQ + k);
-        }
-        dg::pr_cholesky_apply<3>(rec + kGcL, r, z);
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          rec[kGcR + k] = r[k];
-          rec[kGcZ + k] = z[k];
-          rr += r[k] * r[k];
-          rz += r[k] * z[k];
-        }
-        a.part[kPartRR * (size_t)nc + c] = rr;
-        a.part[kPartRZ * (size_t)nc + c] = rz;
-      }
-      grid.sync();
-      double rr, rz;
-      cta_sum2(a.part + kPartRR * (size_t)nc, a.part + kPartRZ * (size_t)nc, nc, sh, &rr, &rz);
-      if (rr <= a.cg_tol2 * bb || it >= a.cg_max_iters) break;
-      beta = rz / rho;
-      rho = rz;
-    }
-  }
+  const GpSchur op{a, tid, nthr, (int)threadIdx.x & 31, tid >> 5, nthr >> 5, 1.0 / (1.0 + st->lam)};
+  const PcgResult res = pcg_run<kGpSolveThreads>(grid, a.part, nc, a.cg_tol2, a.cg_max_iters, sh, op);
   // the trial centres of the views that move (x of a view was last written by this thread, in phase C)
   const int cur = st->cur;
-  if (!reject)
+  if (!res.reject)
     for (int c = tid; c < nc; c += nthr) {
       if (a.list_off[c + 1] == a.list_off[c]) continue;
       const double* x = view_rec(a, c) + kGcX;
@@ -610,8 +548,8 @@ __global__ void __launch_bounds__(kGpSolveThreads) gp_solve_kernel(GpArgs a) {
       for (int k = 0; k < 3; ++k) c1[k] = c0[k] + x[k];
     }
   if (tid == 0) {
-    a.cg_iters[0] += it;
-    if (reject) st->bad = 1;
+    a.cg_iters[0] += res.iters;
+    if (res.reject) st->bad = 1;
   }
 }
 
@@ -715,15 +653,6 @@ __global__ void __launch_bounds__(kGpThreads) gp_finish_obs_kernel(GpArgs a) {
   a.inl_out[r] = th <= a.max_angle ? 1 : 0;          // (false for NaN)
 }
 
-template <typename T>
-T* carve(char*& p, size_t count) {
-  T* out = (T*)p;
-  p += (sizeof(T) * count + 255) / 256 * 256;
-  return out;
-}
-
-int blocks(size_t n, int per) { return (int)((n + per - 1) / per); }
-
 }  // namespace
 
 extern "C" {
@@ -753,57 +682,51 @@ int dgb200_global_positioning_ragged_dev(const int32_t* d_cams, const double* d_
   if (cg_max_iters < 1) return fail(DGB200_E_ARG, "cg_max_iters must be at least 1");
   if (!(cg_tol >= 0.0) || !(cg_tol < INFINITY)) return fail(DGB200_E_ARG, "cg_tol must be a non-negative finite number");
   const cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 0, coop = 0, per_sm = 0;
-  CU(cudaGetDevice(&dev));
-  CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) return fail(DGB200_E_CUDA, "the device does not support cooperative launches");
+  int sms = 0, per_sm = 0;
+  cudaError_t e = cudaSuccess;
+  if (const char* m = coop_sms(&sms, &e)) return fail(DGB200_E_CUDA, m, e);
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_solve_kernel, kGpSolveThreads, 0));
   if (per_sm < 1) return fail(DGB200_E_CUDA, "gp_solve_kernel does not fit on an SM");
   const int n_ranges = obs > 0 ? blocks((size_t)obs, kGpRange) : 1;
   const size_t no = (size_t)(obs > 0 ? obs : 1), nt = (size_t)n_tracks, nc = (size_t)n_cams;
-  size_t bytes = 0;
-  {                                                  // the carve below, counted
-    const size_t d = sizeof(double), i = sizeof(int);
-    const size_t sizes[] = {d * dg::kTrCamStride * nc, d * 6 * nc, d * 6 * nt, d * 2 * no, d * 3 * no,
-                            d * kLoRows * no, d * kLcRows * no, d * dg::kBaTrkStride * nt, d * kGvStride * nt,
-                            d * 3 * nt, d * kGcStride * nc, d * kGpParts * nc, sizeof(BaState), i, i, i * nc, i * nc,
-                            i * no, i * no, i * no, i * no, i * nc * (size_t)n_ranges, i * (nc + 1), i * nt, no};
-    for (size_t s : sizes) bytes += (s + 255) / 256 * 256;
-  }
-  char* ws = nullptr;
-  CU(cudaMallocAsync((void**)&ws, bytes, st));
   GpArgs a;
   a.cams = d_cams; a.pts = d_pts; a.R = d_R; a.K = d_K; a.k_per_camera = k_per_camera; a.n_cams = n_cams;
   a.offsets = d_offsets; a.mask = d_mask; a.n_tracks = n_tracks; a.obs = obs; a.n_ranges = n_ranges;
   a.cg_max_iters = cg_max_iters; a.seed = seed; a.init_scale = init_scale; a.delta = loss_scale;
   a.max_angle = max_angle; a.cg_tol2 = cg_tol * cg_tol;
-  char* p = ws;
-  a.tab = carve<double>(p, dg::kTrCamStride * nc);
-  a.cen = carve<double>(p, 6 * nc);
-  a.Xb = carve<double>(p, 6 * nt);
-  a.dsc = carve<double>(p, 2 * no);
-  a.ray = carve<double>(p, 3 * no);
-  a.lo = carve<double>(p, kLoRows * no);
-  a.lc = carve<double>(p, kLcRows * no);
-  a.trk = carve<double>(p, dg::kBaTrkStride * nt);
-  a.tv = carve<double>(p, kGvStride * nt);
-  a.y = carve<double>(p, 3 * nt);
-  a.rec = carve<double>(p, kGcStride * nc);
-  a.part = carve<double>(p, kGpParts * nc);
-  a.state = carve<BaState>(p, 1);
-  a.cg_iters = carve<int>(p, 1);
-  a.linbad = carve<int>(p, 1);
-  a.parent = carve<int>(p, nc);
-  a.active = carve<int>(p, nc);
-  a.key = carve<int>(p, no);
-  a.track_of = carve<int>(p, no);
-  a.pos_of = carve<int>(p, no);
-  a.ctrk = carve<int>(p, no);
-  a.hist = carve<int>(p, nc * (size_t)n_ranges);
-  a.list_off = carve<int>(p, nc + 1);
-  a.trk_used = carve<int>(p, nt);
-  a.used = carve<unsigned char>(p, no);
+  auto lay_out = [&](char* base) {
+    Carve w{base};
+    a.tab = w.take<double>(dg::kTrCamStride * nc);
+    a.cen = w.take<double>(6 * nc);
+    a.Xb = w.take<double>(6 * nt);
+    a.dsc = w.take<double>(2 * no);
+    a.ray = w.take<double>(3 * no);
+    a.lo = w.take<double>(kLoRows * no);
+    a.lc = w.take<double>(kLcRows * no);
+    a.trk = w.take<double>(dg::kBaTrkStride * nt);
+    a.tv = w.take<double>(kGvStride * nt);
+    a.y = w.take<double>(3 * nt);
+    a.rec = w.take<double>(kGcStride * nc);
+    a.part = w.take<double>(kPcgParts * nc);
+    a.state = w.take<BaState>(1);
+    a.cg_iters = w.take<int>(1);
+    a.linbad = w.take<int>(1);
+    a.parent = w.take<int>(nc);
+    a.active = w.take<int>(nc);
+    a.key = w.take<int>(no);
+    a.track_of = w.take<int>(no);
+    a.pos_of = w.take<int>(no);
+    a.ctrk = w.take<int>(no);
+    a.hist = w.take<int>(nc * (size_t)n_ranges);
+    a.list_off = w.take<int>(nc + 1);
+    a.trk_used = w.take<int>(nt);
+    a.used = w.take<unsigned char>(no);
+    return w.bytes;
+  };
+  char* ws = nullptr;
+  const size_t bytes = lay_out(nullptr);
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
+  lay_out(ws);
   a.t_out = d_t_out; a.X_out = d_X_out; a.comp_out = d_component_out; a.angle_out = d_angle_out;
   a.inl_out = d_inliers_out; a.cost0_out = d_cost0_out; a.cost_out = d_cost_out; a.iters_out = d_iters_out;
   a.n_used_out = d_n_used_out; a.cg_iters_out = d_cg_iters_out;
@@ -812,40 +735,34 @@ int dgb200_global_positioning_ragged_dev(const int32_t* d_cams, const double* d_
   const int obs_grid = blocks(no, kGpThreads), range_grid = blocks((size_t)n_ranges, kGpWarps);
   void* solve_args[] = {&a};
   cudaError_t launch = cudaSuccess;
-#define LG(...)                                   \
-  if (launch == cudaSuccess) {                    \
-    __VA_ARGS__;                                  \
-    launch = cudaGetLastError();                  \
-  }
-  LG(launch = cudaMemsetAsync(a.used, 0, no, st));              // rows outside every span are not used
-  LG(launch = cudaMemsetAsync(a.track_of, 0xff, sizeof(int) * no, st));
-  LG(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nc + 1), st));
-  LG(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nc * (size_t)n_ranges, st));
-  LG((gp_cameras_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
-  LG((gp_mark_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
-  LG((gp_compress_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.used, 0, no, st));              // rows outside every span are not used
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.track_of, 0xff, sizeof(int) * no, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.list_off, 0, sizeof(int) * (nc + 1), st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nc * (size_t)n_ranges, st));
+  ADJ_LAUNCH((gp_cameras_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_mark_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_compress_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
   if (obs > 0) {
-    LG((gp_key_kernel<<<obs_grid, kGpThreads, 0, st>>>(a)));
-    LG((gp_count_kernel<<<range_grid, 32 * kGpWarps, 0, st>>>(a)));
-    LG((gp_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
-    LG((gp_scatter_kernel<<<range_grid, 32 * kGpWarps, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_key_kernel<<<obs_grid, kGpThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_count_kernel<<<range_grid, 32 * kGpWarps, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_scatter_kernel<<<range_grid, 32 * kGpWarps, 0, st>>>(a)));
   }
-  LG((gp_start_views_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
-  LG((gp_start_tracks_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
-  LG((gp_init_kernel<<<1, kBaCta, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_start_views_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_start_tracks_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_init_kernel<<<1, kBaCta, 0, st>>>(a)));
   for (int it = 0; it < max_iters && launch == cudaSuccess; ++it) {
-    LG((gp_linearise_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
-    LG((gp_points_kernel<<<trk_thread_grid, kGpThreads, 0, st>>>(a)));
-    LG((gp_precond_kernel<<<cam_warp_grid, 32 * kGpWarps, 0, st>>>(a)));
-    LG(launch = cudaLaunchCooperativeKernel((const void*)gp_solve_kernel, per_sm * sms, kGpSolveThreads, solve_args, 0,
-                                            st));
-    LG((gp_backsub_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
-    LG((gp_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_linearise_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_points_kernel<<<trk_thread_grid, kGpThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_precond_kernel<<<cam_warp_grid, 32 * kGpWarps, 0, st>>>(a)));
+    ADJ_LAUNCH(launch = cudaLaunchCooperativeKernel((const void*)gp_solve_kernel, per_sm * sms, kGpSolveThreads,
+                                                    solve_args, 0, st));
+    ADJ_LAUNCH((gp_backsub_kernel<<<trk_grid, 32 * kGpWarps, 0, st>>>(a)));
+    ADJ_LAUNCH((gp_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
   }
-  LG((gp_finish_views_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
-  LG((gp_finish_tracks_kernel<<<trk_thread_grid, kGpThreads, 0, st>>>(a)));
-  if (obs > 0) LG((gp_finish_obs_kernel<<<obs_grid, kGpThreads, 0, st>>>(a)));
-#undef LG
+  ADJ_LAUNCH((gp_finish_views_kernel<<<cam_grid, kGpThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((gp_finish_tracks_kernel<<<trk_thread_grid, kGpThreads, 0, st>>>(a)));
+  if (obs > 0) ADJ_LAUNCH((gp_finish_obs_kernel<<<obs_grid, kGpThreads, 0, st>>>(a)));
   CU(cudaFreeAsync(ws, st));
   CU(launch);
   return 0;

@@ -29,9 +29,9 @@
 // After the last iteration ra_finish_edges_kernel and ra_finish_views_kernel write the outputs.
 //
 // One PCG iteration: B, one warp per view: q_v = d_v p_v - sum_{e in v} w_e p_other over the view's list (a root's q_v
-// = p_v), p_v . q_v; C, one thread per view: x += alpha p, r -= alpha q, z = r / d; r . r and r . z.  The dot products
-// are sums of per-view terms that every CTA sums itself in one fixed order, so they do not depend on the grid.  No
-// floating-point atomics anywhere: a rerun gives the same bytes.
+// = p_v), p_v . q_v; C, one thread per view: x += alpha p, r -= alpha q, z = r / d; r . r and r . z.  The loop is
+// pcg_run (pcg_device.h), whose dot products every CTA sums itself in one fixed order, so they do not depend on the
+// grid.  No floating-point atomics anywhere: a rerun gives the same bytes.
 #include <cooperative_groups.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,6 +44,8 @@
 #include "tracks.h"
 #include "device_util.h"
 #include "bundle_adjust_device.h"
+#include "pcg_device.h"
+#include "adjust_host.h"
 
 namespace cg = cooperative_groups;
 
@@ -58,10 +60,11 @@ constexpr int kRaSolveThreads = 256;              // the cooperative kernels
 constexpr int kRaRange = 4096;                    // entries per warp of the counting sort
 constexpr unsigned long long kRaNoEdge = ~0ull;
 
-// One view's record: the Laplacian's diagonal d, then b, x, r, z, p in two buffers and q (3 each)
-constexpr int kRvD = 0, kRvB = 1, kRvX = 4, kRvR = 7, kRvZ = 10, kRvP = 13, kRvQ = 19, kRvStride = 22;
-// The per-view terms of the dot products and the step lengths, kRaParts arrays of n_views
-constexpr int kPartPQ = 0, kPartRR = 1, kPartRZ = 2, kPartBB = 3, kPartStep = 4, kRaParts = 5;
+// One view's record: the Laplacian's diagonal d, then its PCG vectors (pcg_device.h): b, x, r, z, p in two buffers
+// and q (3 each)
+constexpr int kRvD = 0, kRvB = 1, kRvX = 4, kRvP = 13, kRvQ = 19, kRvStride = 22;
+// The per-view terms of the dot products (pcg_device.h), then the step lengths: kRaParts arrays of n_views
+constexpr int kPartStep = kPcgParts, kRaParts = kPcgParts + 1;
 constexpr int kPhaseDone = 2;
 
 struct RaState {
@@ -269,144 +272,86 @@ __global__ void __launch_bounds__(32 * kRaWarps) ra_rhs_kernel(RaArgs a) {
   }
   double* rec = view_rec(a, v);
   rec[kRvD] = d;
-  double rz = 0.0, bb = 0.0;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) {
-    const double z = b[k] / d;
-    rec[kRvB + k] = b[k];
-    rec[kRvX + k] = 0.0;
-    rec[kRvR + k] = b[k];
-    rec[kRvZ + k] = z;
-    rec[kRvP + k] = 0.0;
-    rec[kRvP + 3 + k] = 0.0;
-    rz += b[k] * z;
-    bb += b[k] * b[k];
-  }
-  a.part[kPartRZ * (size_t)a.n_views + v] = rz;
-  a.part[kPartBB * (size_t)a.n_views + v] = bb;
+  const double z[3] = {b[0] / d, b[1] / d, b[2] / d};
+  pcg_start<3>(rec + kRvB, b, z, a.part, a.n_views, v);
 }
 
-// The fixed-order sums over the views of up to two per-view arrays, the same in every CTA: thread t adds views t, t +
-// kRaSolveThreads, ... in turn, then a tree over the threads.  Every thread gets the sums.  (bundle_adjust_pcg.cu's
-// cta_sum2 over its slots.)
-__device__ void cta_sum2(const double* u, const double* v, int n, double* sh, double* su, double* sv) {
-  double x = 0.0, y = 0.0;
-  for (int i = threadIdx.x; i < n; i += kRaSolveThreads) {
-    x += __ldcg(u + i);
-    if (v) y += __ldcg(v + i);
-  }
-  sh[threadIdx.x] = x;
-  sh[kRaSolveThreads + threadIdx.x] = y;
-  __syncthreads();
-  for (int s = kRaSolveThreads / 2; s > 0; s >>= 1) {
-    if ((int)threadIdx.x < s) {
-      sh[threadIdx.x] += sh[threadIdx.x + s];
-      sh[kRaSolveThreads + threadIdx.x] += sh[kRaSolveThreads + threadIdx.x + s];
+// pcg_run's S p and phase C over the views.  product: B, one warp per view, q_v = d_v p_v - sum_e w_e p_other, p_v
+// stored, p_v . q_v.  update: one thread per view.
+struct RaLaplacian {
+  const RaArgs& a;
+  int tid, nthr, lane, warp, nwarps;
+
+  __device__ __forceinline__ void product(cg::grid_group& /*grid*/, int cur, int prev, double beta) const {
+    const int n = a.n_views;
+    for (int v = warp; v < n; v += nwarps) {
+      double acc[3] = {0.0, 0.0, 0.0};
+      const bool pin = pinned(a, v);
+      if (!pin) {
+        const int i0 = a.list_off[v], i1 = a.list_off[v + 1];
+        for (int i = i0 + lane; i < i1; i += 32) {
+          const int entry = a.item[i];
+          const double w = a.er[4 * (size_t)(entry >> 1) + 3];
+          double po[3];
+          pcg_direction<3>(view_rec(a, other_view(a, entry)) + kRvB, prev, beta, po);
+          acc[0] += w * po[0]; acc[1] += w * po[1]; acc[2] += w * po[2];
+        }
+#pragma unroll
+        for (int k = 0; k < 3; ++k) acc[k] = warp_sum(acc[k]);
+      }
+      if (lane == 0) {
+        double p[3];
+        double* rec = view_rec(a, v);
+        pcg_direction<3>(rec + kRvB, prev, beta, p);
+        const double d = rec[kRvD];
+        double pq = 0.0;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const double q = pin ? p[k] : d * p[k] - acc[k];
+          rec[kRvQ + k] = q;
+          rec[kRvP + 3 * cur + k] = p[k];
+          pq += p[k] * q;
+        }
+        a.part[kPartPQ * (size_t)n + v] = pq;
+      }
     }
-    __syncthreads();
   }
-  *su = sh[0];
-  *sv = sh[kRaSolveThreads];
-  __syncthreads();
-}
 
-// p_v = z_v + beta p'_v, p' in buffer `prev`
-__device__ __forceinline__ void direction(const RaArgs& a, int v, int prev, double beta, double* p) {
-  const double* rec = view_rec(a, v);
+  __device__ __forceinline__ void update(int cur, int /*prev*/, double /*beta*/, double alpha) const {
+    const int n = a.n_views;
+    for (int v = tid; v < n; v += nthr) {
+      double* rec = view_rec(a, v);
+      const double d = rec[kRvD];
+      double p[3], q[3];
 #pragma unroll
-  for (int k = 0; k < 3; ++k) p[k] = __ldcg(rec + kRvZ + k) + beta * __ldcg(rec + kRvP + 3 * prev + k);
-}
+      for (int k = 0; k < 3; ++k) {
+        p[k] = __ldcg(rec + kRvP + 3 * cur + k);
+        q[k] = __ldcg(rec + kRvQ + k);
+      }
+      const double2 rz = pcg_update<3>(rec + kRvB, p, q, alpha, [d](const double* r, double* z) {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) z[k] = r[k] / d;
+      });
+      a.part[kPartRR * (size_t)n + v] = rz.x;
+      a.part[kPartRZ * (size_t)n + v] = rz.y;
+    }
+  }
+};
 
-// The PCG loop of one iteration, then the update of every view that is not pinned and its step length |w_v|.  Data
-// written inside the launch is read with __ldcg (L2), as other CTAs wrote it; every CTA computes the same scalars, so
-// every CTA takes the same branches and meets the same grid.sync() calls.
+// The PCG loop of one iteration (pcg_run), then the update of every view that is not pinned and its step length |w_v|
 __global__ void __launch_bounds__(kRaSolveThreads) ra_solve_kernel(RaArgs a) {
   __shared__ double sh[2 * kRaSolveThreads];
   RaState* st = a.state;
   if (st->phase == kPhaseDone) return;               // (grid-uniform: written only by ra_decide_kernel)
   cg::grid_group grid = cg::this_grid();
   const int tid = blockIdx.x * kRaSolveThreads + threadIdx.x, nthr = gridDim.x * kRaSolveThreads;
-  const int lane = threadIdx.x & 31, warp = tid >> 5, nwarps = nthr >> 5;
   const int n = a.n_views;
-  double bb, rho;
-  cta_sum2(a.part + kPartBB * (size_t)n, a.part + kPartRZ * (size_t)n, n, sh, &bb, &rho);
-  int it = 0;
-  bool reject = false;
-  if (bb > 0.0) {
-    double beta = 0.0;
-    for (;;) {
-      const int cur = it & 1, prev = cur ^ 1;
-      // B: q_v = d_v p_v - sum_e w_e p_other
-      for (int v = warp; v < n; v += nwarps) {
-        double acc[3] = {0.0, 0.0, 0.0};
-        const bool pin = pinned(a, v);
-        if (!pin) {
-          const int i0 = a.list_off[v], i1 = a.list_off[v + 1];
-          for (int i = i0 + lane; i < i1; i += 32) {
-            const int entry = a.item[i];
-            const double w = a.er[4 * (size_t)(entry >> 1) + 3];
-            double po[3];
-            direction(a, other_view(a, entry), prev, beta, po);
-            acc[0] += w * po[0]; acc[1] += w * po[1]; acc[2] += w * po[2];
-          }
-#pragma unroll
-          for (int k = 0; k < 3; ++k) acc[k] = warp_sum(acc[k]);
-        }
-        if (lane == 0) {
-          double p[3];
-          direction(a, v, prev, beta, p);
-          double* rec = view_rec(a, v);
-          const double d = rec[kRvD];
-          double pq = 0.0;
-#pragma unroll
-          for (int k = 0; k < 3; ++k) {
-            const double q = pin ? p[k] : d * p[k] - acc[k];
-            rec[kRvQ + k] = q;
-            rec[kRvP + 3 * cur + k] = p[k];
-            pq += p[k] * q;
-          }
-          a.part[kPartPQ * (size_t)n + v] = pq;
-        }
-      }
-      grid.sync();
-      // C: alpha, x, r, z
-      double kappa, unused;
-      cta_sum2(a.part + kPartPQ * (size_t)n, nullptr, n, sh, &kappa, &unused);
-      ++it;
-      if (!(kappa > 0.0) || !finite(kappa)) {
-        reject = it == 1;
-        break;
-      }
-      const double alpha = rho / kappa;
-      for (int v = tid; v < n; v += nthr) {
-        double* rec = view_rec(a, v);
-        const double d = rec[kRvD];
-        double rr = 0.0, rz = 0.0;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-          rec[kRvX + k] = __ldcg(rec + kRvX + k) + alpha * __ldcg(rec + kRvP + 3 * cur + k);
-          const double r = __ldcg(rec + kRvR + k) - alpha * __ldcg(rec + kRvQ + k);
-          const double z = r / d;
-          rec[kRvR + k] = r;
-          rec[kRvZ + k] = z;
-          rr += r * r;
-          rz += r * z;
-        }
-        a.part[kPartRR * (size_t)n + v] = rr;
-        a.part[kPartRZ * (size_t)n + v] = rz;
-      }
-      grid.sync();
-      double rr, rz;
-      cta_sum2(a.part + kPartRR * (size_t)n, a.part + kPartRZ * (size_t)n, n, sh, &rr, &rz);
-      if (rr <= a.cg_tol2 * bb || it >= a.cg_max_iters) break;
-      beta = rz / rho;
-      rho = rz;
-    }
-  }
+  const RaLaplacian op{a, tid, nthr, (int)threadIdx.x & 31, tid >> 5, nthr >> 5};
+  const PcgResult res = pcg_run<kRaSolveThreads>(grid, a.part, n, a.cg_tol2, a.cg_max_iters, sh, op);
   // the update (x of a view was last written by this thread, in phase C)
   for (int v = tid; v < n; v += nthr) {
     double step = 0.0;
-    if (!reject && !pinned(a, v)) {
+    if (!res.reject && !pinned(a, v)) {
       const double* x = view_rec(a, v) + kRvX;
       const double w[3] = {x[0], x[1], x[2]};
       double* R = a.R + 9 * (size_t)v;
@@ -418,8 +363,8 @@ __global__ void __launch_bounds__(kRaSolveThreads) ra_solve_kernel(RaArgs a) {
     a.part[kPartStep * (size_t)n + v] = step;
   }
   if (tid == 0) {
-    st->cg_iters += it;
-    st->reject = reject ? 1 : 0;
+    st->cg_iters += res.iters;
+    st->reject = res.reject ? 1 : 0;
   }
 }
 
@@ -470,15 +415,6 @@ __global__ void __launch_bounds__(kRaThreads) ra_finish_views_kernel(RaArgs a) {
   a.comp_out[v] = a.list_off[v + 1] > a.list_off[v] ? a.parent[v] : -1;
 }
 
-template <typename T>
-T* carve(char*& p, size_t count) {
-  T* out = (T*)p;
-  p += (sizeof(T) * count + 255) / 256 * 256;
-  return out;
-}
-
-int blocks(size_t n, int per) { return (int)((n + per - 1) / per); }
-
 }  // namespace
 
 extern "C" {
@@ -503,11 +439,9 @@ int dgb200_average_rotations_dev(const int32_t* h_pairs, int n_pairs, int n_view
   if (cg_max_iters < 1) return fail(DGB200_E_ARG, "cg_max_iters must be at least 1");
   if (!(cg_tol >= 0.0) || !(cg_tol < INFINITY)) return fail(DGB200_E_ARG, "cg_tol must be a non-negative finite number");
   const cudaStream_t st = (cudaStream_t)stream;
-  int dev = 0, sms = 0, coop = 0, per_sm_tree = 0, per_sm_solve = 0;
-  CU(cudaGetDevice(&dev));
-  CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CU(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) return fail(DGB200_E_CUDA, "the device does not support cooperative launches");
+  int sms = 0, per_sm_tree = 0, per_sm_solve = 0;
+  cudaError_t e = cudaSuccess;
+  if (const char* m = coop_sms(&sms, &e)) return fail(DGB200_E_CUDA, m, e);
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_tree, ra_tree_kernel, kRaSolveThreads, 0));
   CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_solve, ra_solve_kernel, kRaSolveThreads, 0));
   if (per_sm_tree < 1 || per_sm_solve < 1) return fail(DGB200_E_CUDA, "a cooperative kernel does not fit on an SM");
@@ -516,77 +450,69 @@ int dgb200_average_rotations_dev(const int32_t* h_pairs, int n_pairs, int n_view
   int rounds = 0;                                    // ceil(log2 n_views) + 1
   while ((1ll << rounds) < (long long)n_views) ++rounds;
   ++rounds;
-  size_t bytes = 0;
-  {                                                  // the carve below, counted
-    const size_t d = sizeof(double), i = sizeof(int);
-    const size_t sizes[] = {sizeof(int2) * np, d * 9 * np, d * 4 * np, np, np, i * ne, i * ne, i * ne, i * ne,
-                            i * nv * (size_t)n_ranges, i * (nv + 1), i * nv, sizeof(unsigned long long) * nv, i * nv,
-                            i * 3, d * 9 * nv, d * kRvStride * nv, d * kRaParts * nv, sizeof(RaState)};
-    for (size_t s : sizes) bytes += (s + 255) / 256 * 256;
-  }
-  char* ws = nullptr;
-  CU(cudaMallocAsync((void**)&ws, bytes, st));
   RaArgs a;
   a.n_views = n_views; a.n_pairs = n_pairs; a.n_entries = (int)ne; a.n_ranges = n_ranges;
   a.l1_iters = l1_iters; a.max_iters = max_iters; a.cg_max_iters = cg_max_iters;
   a.sig2 = sigma * sigma; a.step_tol = step_tol; a.cg_tol2 = cg_tol * cg_tol;
   a.R_rel = d_R_rel; a.mask = d_mask; a.weights = d_weights;
-  char* p = ws;
-  int2* d_pairs = carve<int2>(p, np);
+  int2* d_pairs = nullptr;
+  auto lay_out = [&](char* base) {
+    Carve w{base};
+    d_pairs = w.take<int2>(np);
+    a.Re = w.take<double>(9 * np);
+    a.er = w.take<double>(4 * np);
+    a.valid = w.take<unsigned char>(np);
+    a.in_tree = w.take<unsigned char>(np);
+    a.key = w.take<int>(ne);
+    a.ent = w.take<int>(ne);
+    a.pos_of = w.take<int>(ne);
+    a.item = w.take<int>(ne);
+    a.hist = w.take<int>(nv * (size_t)n_ranges);
+    a.list_off = w.take<int>(nv + 1);
+    a.parent = w.take<int>(nv);
+    a.best = w.take<unsigned long long>(nv);
+    a.level = w.take<int>(nv);
+    a.flag = w.take<int>(3);
+    a.R = w.take<double>(9 * nv);
+    a.rec = w.take<double>(kRvStride * nv);
+    a.part = w.take<double>(kRaParts * nv);
+    a.state = w.take<RaState>(1);
+    return w.bytes;
+  };
+  char* ws = nullptr;
+  const size_t bytes = lay_out(nullptr);
+  CU(cudaMallocAsync((void**)&ws, bytes, st));
+  lay_out(ws);
   a.pairs = d_pairs;
-  a.Re = carve<double>(p, 9 * np);
-  a.er = carve<double>(p, 4 * np);
-  a.valid = carve<unsigned char>(p, np);
-  a.in_tree = carve<unsigned char>(p, np);
-  a.key = carve<int>(p, ne);
-  a.ent = carve<int>(p, ne);
-  a.pos_of = carve<int>(p, ne);
-  a.item = carve<int>(p, ne);
-  a.hist = carve<int>(p, nv * (size_t)n_ranges);
-  a.list_off = carve<int>(p, nv + 1);
-  a.parent = carve<int>(p, nv);
-  a.best = carve<unsigned long long>(p, nv);
-  a.level = carve<int>(p, nv);
-  a.flag = carve<int>(p, 3);
-  a.R = carve<double>(p, 9 * nv);
-  a.rec = carve<double>(p, kRvStride * nv);
-  a.part = carve<double>(p, kRaParts * nv);
-  a.state = carve<RaState>(p, 1);
   a.R_out = d_R_out; a.comp_out = d_component_out; a.res_out = d_residual_out; a.iters_out = d_iters_out;
   a.cg_iters_out = d_cg_iters_out;
   const int edge_grid = blocks(np, kRaThreads), view_grid = blocks(nv, kRaThreads);
   const int range_grid = blocks((size_t)n_ranges, kRaWarps), warp_grid = blocks(nv, kRaWarps);
   void* coop_args[] = {&a};
   cudaError_t launch = cudaSuccess;
-#define LR(...)                                   \
-  if (launch == cudaSuccess) {                    \
-    __VA_ARGS__;                                  \
-    launch = cudaGetLastError();                  \
-  }
-  LR(launch = cudaMemcpyAsync(d_pairs, h_pairs, sizeof(int2) * np, cudaMemcpyHostToDevice, st));
-  LR(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nv * (size_t)n_ranges, st));
-  LR((ra_edges_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
-  LR((ra_views_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
-  LR((ra_count_kernel<<<range_grid, 32 * kRaWarps, 0, st>>>(a)));
-  LR((ra_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
-  LR((ra_scatter_kernel<<<range_grid, 32 * kRaWarps, 0, st>>>(a)));
+  ADJ_LAUNCH(launch = cudaMemcpyAsync(d_pairs, h_pairs, sizeof(int2) * np, cudaMemcpyHostToDevice, st));
+  ADJ_LAUNCH(launch = cudaMemsetAsync(a.hist, 0, sizeof(int) * nv * (size_t)n_ranges, st));
+  ADJ_LAUNCH((ra_edges_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((ra_views_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((ra_count_kernel<<<range_grid, 32 * kRaWarps, 0, st>>>(a)));
+  ADJ_LAUNCH((ra_scan_kernel<<<1, kBaCta, 0, st>>>(a)));
+  ADJ_LAUNCH((ra_scatter_kernel<<<range_grid, 32 * kRaWarps, 0, st>>>(a)));
   for (int r = 0; r < rounds; ++r) {
-    LR((ra_min_edge_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
-    LR((ra_hook_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
-    LR((ra_compress_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ra_min_edge_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ra_hook_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ra_compress_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
   }
-  LR(launch = cudaLaunchCooperativeKernel((const void*)ra_tree_kernel, per_sm_tree * sms, kRaSolveThreads, coop_args,
-                                          0, st));
+  ADJ_LAUNCH(launch = cudaLaunchCooperativeKernel((const void*)ra_tree_kernel, per_sm_tree * sms, kRaSolveThreads,
+                                                  coop_args, 0, st));
   for (int it = 0; it < l1_iters + max_iters && launch == cudaSuccess; ++it) {
-    LR((ra_residual_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
-    LR((ra_rhs_kernel<<<warp_grid, 32 * kRaWarps, 0, st>>>(a)));
-    LR(launch = cudaLaunchCooperativeKernel((const void*)ra_solve_kernel, per_sm_solve * sms, kRaSolveThreads,
-                                            coop_args, 0, st));
-    LR((ra_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
+    ADJ_LAUNCH((ra_residual_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
+    ADJ_LAUNCH((ra_rhs_kernel<<<warp_grid, 32 * kRaWarps, 0, st>>>(a)));
+    ADJ_LAUNCH(launch = cudaLaunchCooperativeKernel((const void*)ra_solve_kernel, per_sm_solve * sms, kRaSolveThreads,
+                                                    coop_args, 0, st));
+    ADJ_LAUNCH((ra_decide_kernel<<<1, kBaCta, 0, st>>>(a)));
   }
-  LR((ra_finish_edges_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
-  LR((ra_finish_views_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
-#undef LR
+  ADJ_LAUNCH((ra_finish_edges_kernel<<<edge_grid, kRaThreads, 0, st>>>(a)));
+  ADJ_LAUNCH((ra_finish_views_kernel<<<view_grid, kRaThreads, 0, st>>>(a)));
   CU(cudaFreeAsync(ws, st));
   CU(launch);
   return 0;
