@@ -18,6 +18,10 @@
                                             ->  every view's rotation averaged over the view graph (CUDA)
                                             ->  every view's position and every track's point from the rotations
                                             ->  tracks triangulated on the positioning's inliers, bundle-adjusted
+    and many views whose focal length is not known:
+                                            ->  the camera's focal length from the pairs' F (view-graph calibration)
+                                            ->  pose, rotations on the calibration's inlier pairs, positions, tracks
+                                            ->  bundle adjustment that also refines the intrinsics
 
 The reference does the matching with cv2.BFMatcher on the host (simple-example.py:46-53) and copies the tentative
 correspondences into numpy arrays; here nothing visits the host between the descriptors and the inlier mask.
@@ -33,7 +37,7 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pydegensac_b200 as pydegensac
-from pydegensac_b200.matching import (average_rotations, build_tracks_ragged, global_positioning_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
+from pydegensac_b200.matching import (average_rotations, build_tracks_ragged, calibrate_view_graph, global_positioning_ragged, bundle_adjust_intrinsics_ragged, bundle_adjust_pcg_ragged,
                                       find_absolute_pose_ragged, undistort_points,
                                       match_descriptors, match_descriptors_batch, trim_tracks,
                                       match_descriptors_guided, pose_from_fundamental, pose_from_fundamental_ragged,
@@ -366,6 +370,63 @@ def global_reconstruction(dev, K):
     report_global_reconstruction(scene, global_reconstruction_run(dev, K, scene))
 
 
+def uncalibrated_reconstruction_run(dev, scene, k_start=(768.0, 320.0, 240.0, 0.0, 0.0)):
+    """Global SfM on the path scene without K from outside and with no host read: every pair matched and verified by the
+    ragged F RANSAC; one camera group's focal length calibrated from the pairs' F, starting from k_start (f0 = 1.2
+    max(w, h), the usual guess without EXIF; the planted f is 800); K built from the result on the device; pose and
+    refinement with it; the rotations averaged over the calibration's inlier pairs; tracks, positions and triangulation;
+    one bundle adjustment that also refines the intrinsics, from the calibrated ones.  Returns (calibration, rotation
+    averaging, positioning, triangulation, bundle adjustment)"""
+    _, Rs, _, kps, descs, pairs = scene
+    f64, i32 = torch.float64, torch.int32
+    m = match_descriptors_batch(descs, pairs, kps, ratio=0.9, mutual=True)
+    seeds = torch.arange(len(pairs), dtype=torch.int64, device=dev)
+    F, mask = pydegensac.findFundamentalMatrixBatch(m.pts1, m.pts2, 0.5, 0.999, 10000, seeds=seeds, offsets=m.offsets,
+                                                    n_max=m.n_max)
+    groups = torch.zeros(len(Rs), dtype=i32, device=dev)            # one camera took every view
+    # filled on the device from Python scalars (a fill, not a copy from the host, which would synchronise)
+    k0 = torch.stack([torch.full((), v, dtype=f64, device=dev) for v in k_start]).view(1, 5)
+    cal = calibrate_view_graph(pairs, F, groups, k0)
+    k = cal.intrinsics[0]
+    zero, one = torch.zeros((), dtype=f64, device=dev), torch.ones((), dtype=f64, device=dev)
+    K = torch.stack([k[0], zero, k[1], zero, k[0], k[2], zero, zero, one]).view(3, 3)
+    pose = pose_from_fundamental_ragged(F, K, K, m.pts1, m.pts2, m.offsets, mask)
+    fine = refine_pose_ragged(pose.R, pose.t, K, K, m.pts1, m.pts2, m.offsets, pose.in_front, px_th=1.0)
+    ra = average_rotations(pairs, fine.R, len(Rs), mask=cal.inliers, weights=pose.good)
+    tk = build_tracks_ragged([len(k) for k in kps], pairs, m.idx1, m.idx2, m.offsets, mask, kps=kps)
+    gpos = global_positioning_ragged(tk.cams, tk.pts, ra.R, K, tk.offsets)
+    tr = triangulate_tracks_ragged(tk.cams, tk.pts, ra.R, gpos.t, K, tk.offsets, mask=gpos.inliers, px_th=3.0)
+    ba = bundle_adjust_intrinsics_ragged(tk.cams, tk.pts, ra.R, gpos.t, groups, cal.intrinsics, tk.offsets, tr.X,
+                                         mask=tr.mask, loss_scale=1.0)
+    return cal, ra, gpos, tr, ba
+
+
+def report_uncalibrated_reconstruction(scene, out, f_true=800.0, f_start=768.0):
+    """Prints the focal error at the start, after calibration and after bundle adjustment, and the largest centre and
+    rotation errors after bundle adjustment; returns (relative focal error after calibration, after BA, largest centre
+    error, largest rotation error in degrees)"""
+    _, Rs, ts, _, _, pairs = scene
+    cal, ra, gpos, tr, ba = out
+    f_cal, f_ba = float(cal.intrinsics[0, 0]), float(ba.intrinsics[0, 0])
+    c1, r1 = similarity_errors(ba.R.cpu().numpy(), ba.t.cpu().numpy(), Rs, ts)
+    print("uncalibrated reconstruction of %d views: calibration over %d of %d pairs in %d trial steps (%d CG), %d "
+          "inlier pairs; bundle adjustment with the intrinsics in %d trial steps"
+          % (len(Rs), int(cal.n_used[0]), len(pairs), int(cal.iters[0]), int(cal.cg_iters[0]), int(cal.inliers.sum()),
+             int(ba.iters[0])))
+    e = [abs(f - f_true) / f_true for f in (f_start, f_cal, f_ba)]
+    print("  focal length %.1f -> %.2f calibrated -> %.2f adjusted (planted %.0f: error %.2f %% -> %.3f %% -> %.3f %%);"
+          " largest centre error %.2e (baseline 0.3), rotation error %.3f deg"
+          % (f_start, f_cal, f_ba, f_true, 100 * e[0], 100 * e[1], 100 * e[2], c1.max(), r1.max()))
+    return e[1], e[2], c1.max(), r1.max()
+
+
+def uncalibrated_reconstruction(dev):
+    """The path scene's 100 views from descriptors to a bundle-adjusted reconstruction, with neither K nor poses from
+    outside"""
+    scene = path_scene(dev)
+    report_uncalibrated_reconstruction(scene, uncalibrated_reconstruction_run(dev, scene))
+
+
 def self_calibration(dev, n_img=20, n_pts=4000, seed=9):
     """Views through a lens with radial distortion (f = 520, k1 = -0.08, k2 = 0.01), known tracks, and a start with a
     focal length 5 % off and no distortion: undistort, triangulate, adjust poses, points and the intrinsics of the one
@@ -463,6 +524,7 @@ def main():
     rotations_from_view_graph(dev, K)
     global_reconstruction(dev, K)
     self_calibration(dev)
+    uncalibrated_reconstruction(dev)
 
 
 if __name__ == "__main__":

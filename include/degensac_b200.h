@@ -690,6 +690,56 @@ int dgb200_build_tracks_ragged_dev(const int32_t* img_offsets, int n_images, con
                                    int32_t* d_cams_out, int32_t* d_kp_out, double* d_pts_out, int32_t* d_track_of_out,
                                    int32_t* d_stats_out, void* stream);
 const char* dgb200_tracks_last_error(void);
+/* View-graph calibration (GLOMAP's first step, before rotation averaging): each camera group's focal length from the
+ * fundamental matrices of the verified pairs, and the pairs whose F does not agree with the result.
+ *   Edges: h_pairs [n_pairs][2] is a HOST table of (i, j) over n_views views; d_F float64 [n_pairs][9] row-major with
+ *   x_j^T F_e x_i = 0 (what dgb200_find_fundamental_batch returns for pts1 from view i and pts2 from view j, the
+ *   convention of dgb200_pose_from_fundamental_ragged_dev); d_mask uint8 [n_pairs] or NULL (every edge).  d_groups
+ *   int32 [n_views] the camera group g(v) of each view; d_intrinsics float64 [n_groups][5] each group's start (f0, cx,
+ *   cy, k1, k2), the RADIAL row of dgb200_bundle_adjust_intrinsics_ragged_dev; K0 = [[f0, 0, cx], [0, f0, cy],
+ *   [0, 0, 1]].  k1 and k2 play no part: F is taken as the pinhole F of the pixels given.
+ *   1 Unknowns: theta_g per group, f_g = f0_g exp(theta_g); the principal point is held.
+ *   2 Constants of an edge: G = K0_{g(j)}^T F_e K0_{g(i)} scaled to unit Frobenius norm, G = U S V^T by
+ *     dg::svd3_onesided with s1 >= s2 >= s3, v1, v2 from V and u_k = G v_k / s_k.  With w(theta) = diag(e^{2 theta},
+ *     e^{2 theta}, 1), the simplified Kruppa equations (Hartley, PAMI 1997) compare A = (s1^2 v1^T w_i v1, s1 s2 v1^T
+ *     w_i v2, s2^2 v2^T w_i v2) and B = (u2^T w_j u2, -u1^T w_j u2, u1^T w_j u1); A_k = alpha_k e^{2 theta_i} + beta_k
+ *     and B_k = gamma_k e^{2 theta_j} + delta_k, 12 constants per edge.
+ *   3 Used edge: i != j, both views' groups in [0, n_groups), the mask set, F finite, both groups' intrinsics finite
+ *     with f0 > 0, and s2 > 1e-6 s1.
+ *   4 Residuals, both in [-1, 1] and unchanged when F is scaled: r1 = (A0 B2 - A2 B0) / (A0 B2 + A2 B0) and r2 =
+ *     (A1 / sqrt(A0 A2) - B1 / sqrt(B0 B2)) / 2; both are 0 exactly when the Kruppa equations hold.  The sign of r2
+ *     follows the singular vectors' signs; s_e = r1^2 + r2^2 and the steps do not.
+ *   5 Cost sum_e rho(s_e), rho the Cauchy loss sig2 log(1 + s / sig2) with sig2 = loss_scale^2 and IRLS weight
+ *     1 / (1 + s / sig2) (the bundle adjustments'); loss_scale = 0: the squared loss.
+ *   6 Levenberg-Marquardt from theta = 0 with the schedule and stopping rules of dgb200_bundle_adjust_ragged_dev: each
+ *     trial step solves (H + lambda diag H) x = -g, H = sum J_e^T w_e J_e and g = sum J_e^T w_e r_e, by Jacobi-
+ *     preconditioned CG over the groups with the stopping rules of dgb200_bundle_adjust_pcg_ragged_dev (a first p . q
+ *     that is not positive rejects the step).  An edge whose views share a group contributes one column, the sum of its
+ *     two.  A group without a used edge is pinned at theta = 0.  A trial point where an edge's s is not finite costs
+ *     +inf.
+ * Outputs: d_intrinsics_out float64 [n_groups][5]: a group is refined when it has a used edge and 1 / max_ratio <= f
+ * / f0 <= max_ratio, and then its row is the input's with f = f0 exp(theta); any other group's row is the input's, bit
+ * for bit.  d_refined_out uint8 [n_groups]; d_error_out float64 [n_pairs] sqrt(s_e) at the output intrinsics (NaN for
+ * an edge that is not used); d_inliers_out uint8 [n_pairs]: used with error <= max_error; d_cost0_out, d_cost_out
+ * float64 [1] the cost at theta = 0 and at the last accepted step; d_iters_out (trial steps), d_n_used_out (used
+ * edges), d_cg_iters_out (CG iterations, summed) int32 [1].
+ * Determinism: no floating-point atomics; every sum has a fixed order that does not depend on the launch grid (a
+ * group's list is summed in chunks of 256 entries, then the chunks in order), so a rerun gives the same bytes.  A null
+ * required buffer (d_mask is not), n_views, n_pairs or n_groups < 1, a null h_pairs, a view index outside [0,
+ * n_views), loss_scale or max_error not a non-negative finite number, max_ratio not a finite number >= 1, negative
+ * max_iters, cg_max_iters < 1 or cg_tol not a non-negative finite number returns DGB200_E_ARG before any CUDA call;
+ * the message is dgb200_view_graph_calibration_last_error()'s.  Asynchronous on `stream`: a copy of h_pairs, 9
+ * launches, 6 per trial step whatever cg_max_iters is (the CG loop is one cooperative launch sized by the occupancy
+ * API; every kernel returns at once once the call has stopped) and 2 for the outputs, with a stream-ordered workspace
+ * (cudaMallocAsync / cudaFreeAsync); nothing is read back. */
+int dgb200_calibrate_view_graph_dev(const int32_t* h_pairs, int n_pairs, int n_views, const double* d_F,
+                                    const uint8_t* d_mask, const int32_t* d_groups, const double* d_intrinsics,
+                                    int n_groups, double loss_scale, double max_error, double max_ratio, int max_iters,
+                                    int cg_max_iters, double cg_tol, double* d_intrinsics_out, uint8_t* d_refined_out,
+                                    double* d_error_out, uint8_t* d_inliers_out, double* d_cost0_out,
+                                    double* d_cost_out, int32_t* d_iters_out, int32_t* d_n_used_out,
+                                    int32_t* d_cg_iters_out, void* stream);
+const char* dgb200_view_graph_calibration_last_error(void);
 /* Rotation averaging over a view graph (the first step of global SfM, as GLOMAP's rotation averager): a world rotation
  * for every view from the relative rotations of its verified pairs.  Translations are neither used nor produced.
  *   Edges: h_pairs [n_pairs][2] is a HOST table of (i, j), as dgb200_match_descriptors_batch_dev takes it; d_R_rel

@@ -102,6 +102,9 @@ def lib():
                                                            cd, ci, cd, ci, cd, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp,
                                                            vp]
         L.dgb200_global_positioning_last_error.restype = ctypes.c_char_p
+        L.dgb200_calibrate_view_graph_dev.argtypes = [i32, ci, ci, vp, vp, vp, vp, ci, cd, cd, cd, ci, ci, cd, vp, vp,
+                                                      vp, vp, vp, vp, vp, vp, vp, vp]
+        L.dgb200_view_graph_calibration_last_error.restype = ctypes.c_char_p
         L.dgb200_nullspace_qr7x9_batch_dev.argtypes = [vp, vp, vp, ci, vp]
         L.dgb200_frontend_last_error.restype = ctypes.c_char_p
         L.dgb200_last_error.restype = ctypes.c_char_p

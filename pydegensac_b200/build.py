@@ -40,11 +40,12 @@ def build_cuda(force=False, verbose=False):
     src8 = os.path.join(CSRC, "bundle_adjust_intrinsics.cu")  # bundle adjustment with intrinsics, undistortion
     src9 = os.path.join(CSRC, "rotation_averaging.cu")  # world rotations of many views from their relative rotations
     src10 = os.path.join(CSRC, "global_positioning.cu")  # the views' centres and the tracks' points from the rotations
+    src11 = os.path.join(CSRC, "view_graph_calibration.cu")  # the groups' focal lengths from the pairs' F
     if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest(_csrc_files()):
         return LIB
     nvcc = os.environ.get("NVCC", "nvcc")
     cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3, src4, src5, src6,
-                                                                                 src7, src8, src9, src10]
+                                                                                 src7, src8, src9, src10, src11]
     subprocess.check_call(cmd)
     return LIB
 

@@ -66,6 +66,11 @@ A world rotation for every view from the relative rotations of the verified pair
 graph: a maximum-spanning-tree start ranked by the pairs' support, then robust IRLS); the translations are not estimated:
 
     ra = average_rotations(pairs, fine.R, n_views, weights=pose.good)
+
+Before that, for images whose intrinsics are not known, each camera group's focal length from the pairs' fundamental
+matrices (view-graph calibration: robust Levenberg-Marquardt on the Kruppa residuals); its inliers gate the rotations:
+
+    cal = calibrate_view_graph(pairs, F, groups, intrinsics)
 """
 import collections
 import ctypes
@@ -91,6 +96,8 @@ BundleAdjustmentIntrinsics = collections.namedtuple("BundleAdjustmentIntrinsics"
                                                     "R t X intrinsics mask cost0 cost iters n_used cg_iters")
 TrackSet = collections.namedtuple("TrackSet", "offsets cams kp pts track_of stats")
 RotationAveraging = collections.namedtuple("RotationAveraging", "R component residual iters cg_iters")
+ViewGraphCalibration = collections.namedtuple("ViewGraphCalibration",
+                                              "intrinsics refined error inliers cost0 cost iters n_used cg_iters")
 GlobalPositioning = collections.namedtuple("GlobalPositioning",
                                            "t X component angle inliers cost0 cost iters n_used cg_iters")
 HomographyPose = collections.namedtuple("HomographyPose",
@@ -1078,6 +1085,74 @@ def trim_tracks(ts):
     T, n = (int(v) for v in ts.stats[:2].tolist())
     return TrackSet(ts.offsets[:T + 1], ts.cams[:n], ts.kp[:n], ts.pts[:n] if ts.pts is not None else None,
                     ts.track_of, ts.stats)
+
+
+def calibrate_view_graph(pairs, F, groups, intrinsics, mask=None, loss_scale=1e-2, max_error=1e-2, max_ratio=10.0,
+                         max_iters=100, cg_max_iters=500, cg_tol=1e-6):
+    """Calibrate the view graph: each camera group's focal length from the fundamental matrices of the verified pairs,
+    and the pairs whose F agrees with the result (GLOMAP's view-graph calibration, on the device), for images whose
+    intrinsics are not known.
+
+    pairs: a HOST [P,2] table of (i, j) over the C views, as average_rotations takes it.  F: a CUDA float tensor [P,3,3]
+    or [P,9] (used in float64) with x_j^T F x_i = 0, what findFundamentalMatrixBatch returns with pts1 from view i and
+    pts2 from view j.  groups: int32 [C] CUDA tensor, each view's row of intrinsics; intrinsics: a floating [G,5] CUDA
+    tensor of each group's start (f0, cx, cy, k1, k2), the RADIAL row of bundle_adjust_intrinsics_ragged (1.2 max(w, h)
+    is a usual f0 without EXIF).  mask: [P] bool / uint8 or None (every pair).
+    Each group's f = f0 exp(theta) moves, its principal point is held, k1 and k2 are passed through (F is taken as the
+    pinhole F of the pixels given).  An edge is used when i != j, its mask is set, F is finite, both groups' intrinsics
+    are finite with f0 > 0 and s2 > 1e-6 s1 for the singular values of K0_j^T F K0_i.  Each used edge has two residuals
+    of the simplified Kruppa equations in [-1, 1]; Levenberg-Marquardt from theta = 0 minimises the sum of their Cauchy
+    loss of scale loss_scale (0: the squared loss) for at most max_iters trial steps, each solved by Jacobi-
+    preconditioned CG over the groups (cg_max_iters, cg_tol).  A group without a used edge keeps theta = 0.  The
+    estimator is specified in include/degensac_b200.h.
+    Returns ViewGraphCalibration(intrinsics, refined, error, inliers, cost0, cost, iters, n_used, cg_iters):
+    intrinsics [G,5] float64, with f refined where 1 / max_ratio <= f / f0 <= max_ratio on a group with a used edge and
+    every other row bit-identical to the input; refined [G] bool; error [P] float64 the edge's residual norm at those
+    intrinsics (NaN for an edge that is not used); inliers [P] bool, the used edges with error <= max_error, the mask
+    that average_rotations takes next; cost0, cost [1] float64; iters, n_used, cg_iters [1] int32.  Asynchronous,
+    nothing is read back."""
+    import torch
+    named = (("F", F), ("groups", groups), ("intrinsics", intrinsics))
+    _check_tensors(named, mask)
+    _check_int32("groups", groups)
+    if groups.dim() != 1 or groups.shape[0] < 1:
+        raise ValueError("groups must be [C] with C >= 1, not %s" % list(groups.shape))
+    C = int(groups.shape[0])
+    G = _check_groups(groups, intrinsics, C)
+    pairs = _host_pairs(pairs)
+    pr = np.ascontiguousarray(_check_pair_table(pairs, C), dtype=np.int32)
+    P = len(pr)
+    if _check_model("F", F) != P:
+        raise ValueError("F must hold one matrix per pair (%d), not %d" % (P, int(F.shape[0])))
+    _check_floating((("F", F), ("intrinsics", intrinsics)))
+    _check_mask(mask, "P", P)
+    loss_scale, max_error, max_ratio, cg_tol = float(loss_scale), float(max_error), float(max_ratio), float(cg_tol)
+    for nm, v in (("loss_scale", loss_scale), ("max_error", max_error), ("cg_tol", cg_tol)):
+        if not 0.0 <= v < float("inf"):
+            raise ValueError("%s must be a non-negative finite number, not %r" % (nm, v))
+    if not 1.0 <= max_ratio < float("inf"):
+        raise ValueError("max_ratio must be a finite number >= 1, not %r" % (max_ratio,))
+    max_iters = _check_count("max_iters", max_iters, 0)
+    cg_max_iters = _check_count("cg_max_iters", cg_max_iters, 1)
+    dev = _check_device(named, mask)
+    Fc, kc = _f64(F, intrinsics)
+    f64, i32 = torch.float64, torch.int32
+    L = _cabi.lib()
+    ko = torch.empty((G, 5), dtype=f64, device=dev)
+    ref = torch.empty(G, dtype=torch.uint8, device=dev)
+    err = torch.empty(P, dtype=f64, device=dev)
+    inl = torch.empty(P, dtype=torch.uint8, device=dev)
+    cost0 = torch.empty(1, dtype=f64, device=dev)
+    cost = torch.empty(1, dtype=f64, device=dev)
+    iters = torch.empty(1, dtype=i32, device=dev)
+    n_used = torch.empty(1, dtype=i32, device=dev)
+    cg_iters = torch.empty(1, dtype=i32, device=dev)
+    _call(L.dgb200_calibrate_view_graph_dev, L.dgb200_view_graph_calibration_last_error, dev,
+          pr.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), P, C, Fc, _mask_u8(mask), groups.contiguous(), kc, G,
+          loss_scale, max_error, max_ratio, max_iters, cg_max_iters, cg_tol, ko, ref, err, inl, cost0, cost, iters,
+          n_used, cg_iters)
+    return ViewGraphCalibration(ko, ref.view(torch.bool), err, inl.view(torch.bool), cost0, cost, iters, n_used,
+                                cg_iters)
 
 
 def average_rotations(pairs, R_rel, n_views, mask=None, weights=None, sigma=math.radians(5.0), l1_iters=5,
