@@ -445,6 +445,47 @@ int dgb200_find_absolute_pose_ragged_dev(const double* d_x, const double* d_X, c
                                          uint8_t* d_mask_out, int32_t* d_n_inliers_out, int32_t* d_iters_out,
                                          double* d_cost0_out, double* d_cost_out, void* stream);
 const char* dgb200_absolute_pose_last_error(void);
+/* Relative pose of calibrated image pairs (cv2.findEssentialMat for ragged batches): five-point MSAC-RANSAC with
+ * local optimisation.  Pair p owns rows d_offsets[p] .. d_offsets[p+1]-1 of d_x1 / d_x2 [rows][2] (pixels in images 1
+ * and 2, x2^T F x1 = 0); d_K1 / d_K2 [9] row-major, shared (k_per_pair = 0) or [n_pairs][9] (k_per_pair = 1);
+ * d_seeds [n_pairs] the seeds of the pairs' Philox sample streams; d_mask [rows] or NULL (every row).
+ *   usable rows: mask != 0 and four finite coordinates, in row order (n of them); n < 5: no model.
+ *   iteration k = 1, 2, ...: minimal_sample<5>(seed, k, n) over the usable rows; the five-point solver (Nistér, in
+ *   Stewénius' formulation: null space, ten cubic constraints, 10 x 20 elimination, Sturm-isolated real roots of the
+ *   degree-10 polynomial refined by a fixed number of bisections, a few Gauss-Newton steps on the constraints) on
+ *   K1^-1 [x1, 1] and K2^-1 [x2, 1] gives 0 to 10 essential matrices E (a degenerate sample gives none and still
+ *   counts as an iteration).  Each is scored through F = K2^-T E K1^-1 at unit norm: MSAC cost sum min(e^2, px_th^2)
+ *   over the usable rows, e^2 the Sampson error in pixels, inlier when e^2 < px_th^2 (the rule of the F RANSAC, so
+ *   the two masks compare).  A strictly lower cost replaces the best model.  Iteration k + 1 runs while
+ *   k < N_req = min(max_iters, ceil(log(1 - conf) / log1p(-w^5))), w = inliers / n of the best model (max_iters
+ *   without a model or with conf = 1; k itself when w = 1).
+ *   local optimisation, when refine_iters > 0 and the best model has at least 6 inliers: the start is one
+ *   decomposition E ~ [t]x R (any of the four gives +-E, and the Sampson error ignores the sign); up to 3 rounds of
+ *   Levenberg-Marquardt over (R, t), |t| = 1, on the inliers (the rows, solve and step of
+ *   dgb200_refine_pose_ragged_dev, at most refine_iters trial steps, R re-orthonormalised when an accepted step left
+ *   |R R^T - I| above 1e-12), each followed by a re-selection of the inliers under E = [t]x R; it stops when the
+ *   inlier set does not change (or has fewer than 6 rows).  Its model replaces the RANSAC model only when its MSAC
+ *   cost is <= the RANSAC model's.
+ * The sums of a pair are reduced in a fixed order without atomics: its result does not depend on the batch or the run.
+ * Outputs per pair: d_E_out [9] the essential matrix at unit norm; d_F_out [9] = K2^-T E K1^-1 at unit norm (what
+ * dgb200_pose_from_fundamental_ragged_dev, dgb200_refine_pose_ragged_dev and guided matching take); d_n_inliers_out its
+ * inliers; d_iters_out the RANSAC iterations drawn; d_cost0_out the MSAC cost of the RANSAC model and d_cost_out that
+ * of the output model (cost <= cost0).  d_mask_out [rows]: 1 for the inliers of the output model, 0 for every other
+ * row of the pair.  No R and t are returned: dgb200_pose_from_fundamental_ragged_dev makes the cheirality vote on F.
+ * Pairs without a model (n < 5, or no sample gave a solution): E = F = 0, n_inliers = 0, iters the iterations drawn,
+ * NaN costs, mask rows 0.  Offsets that decrease, are negative or pass `rows`: the same with iters = 0, no row read or
+ * written.  d_mask may be NULL; d_x1, d_x2 and d_mask_out may be NULL when rows = 0; every other buffer is required.
+ * A null required buffer, n_pairs < 1, rows < 0, px_th not a positive finite number, conf outside (0, 1],
+ * max_iters < 1 or refine_iters < 0 returns DGB200_E_ARG before any launch; the message is
+ * dgb200_essential_last_error()'s.  Asynchronous on `stream`: one kernel and a stream-ordered workspace of 4 bytes per
+ * row (cudaMallocAsync / cudaFreeAsync), nothing read back. */
+int dgb200_find_essential_ragged_dev(const double* d_x1, const double* d_x2, const double* d_K1, const double* d_K2,
+                                     int k_per_pair, const int32_t* d_offsets, int n_pairs, int rows,
+                                     const uint8_t* d_mask, double px_th, double conf, int max_iters, int refine_iters,
+                                     const uint64_t* d_seeds, double* d_E_out, double* d_F_out, uint8_t* d_mask_out,
+                                     int32_t* d_n_inliers_out, int32_t* d_iters_out, double* d_cost0_out,
+                                     double* d_cost_out, void* stream);
+const char* dgb200_essential_last_error(void);
 /* Triangulation of tracks across registered views (the step after registering a view in an incremental
  * reconstruction) over a RAGGED batch of tracks: track j owns observations d_offsets[j] .. d_offsets[j+1]-1, each a
  * camera index d_cams [obs] and a pixel d_pts [obs][2].  Camera c has the pose d_R [n_cams][9] (row-major),

@@ -77,6 +77,9 @@ def lib():
         L.dgb200_find_absolute_pose_ragged_dev.argtypes = [vp, vp, vp, ci, vp, ci, ci, vp, cd, cd, ci, ci, vp, vp, vp,
                                                            vp, vp, vp, vp, vp, vp]
         L.dgb200_absolute_pose_last_error.restype = ctypes.c_char_p
+        L.dgb200_find_essential_ragged_dev.argtypes = [vp, vp, vp, vp, ci, vp, ci, ci, vp, cd, cd, ci, ci, vp, vp, vp,
+                                                       vp, vp, vp, vp, vp, vp]
+        L.dgb200_essential_last_error.restype = ctypes.c_char_p
         L.dgb200_triangulate_tracks_ragged_dev.argtypes = [vp, vp, vp, vp, vp, ci, ci, vp, ci, ci, vp, cd, cd, cd, ci, ci,
                                                            vp, vp, vp, vp, vp, vp, vp, vp, vp]
         L.dgb200_triangulate_last_error.restype = ctypes.c_char_p

@@ -41,11 +41,12 @@ def build_cuda(force=False, verbose=False):
     src9 = os.path.join(CSRC, "rotation_averaging.cu")  # world rotations of many views from their relative rotations
     src10 = os.path.join(CSRC, "global_positioning.cu")  # the views' centres and the tracks' points from the rotations
     src11 = os.path.join(CSRC, "view_graph_calibration.cu")  # the groups' focal lengths from the pairs' F
+    src12 = os.path.join(CSRC, "essential.cu")     # five-point RANSAC: relative pose of calibrated pairs
     if not force and os.path.exists(LIB) and os.path.getmtime(LIB) >= _newest(_csrc_files()):
         return LIB
     nvcc = os.environ.get("NVCC", "nvcc")
     cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", LIB, src, src2, src3, src4, src5, src6,
-                                                                                 src7, src8, src9, src10, src11]
+                                                                                 src7, src8, src9, src10, src11, src12]
     subprocess.check_call(cmd)
     return LIB
 

@@ -45,6 +45,12 @@ matrices), then the guided re-match in the band of the refined F:
     fine_f = refine_fundamental_ragged(F, m.pts1, m.pts2, m.offsets, mask, px_th=1.0)
     g = match_descriptors_guided(descs, pairs, kps, fine_f.F, 1.0, guide="F")
 
+Calibrated pairs verified by the five-point solver instead of the 7-point F (essential-matrix RANSAC,
+cv2.findEssentialMat); its F goes on to the pose:
+
+    ess = find_essential_ragged(m.pts1, m.pts2, K1, K2, m.offsets, px_th=1.0)
+    pose = pose_from_fundamental_ragged(ess.F, K1, K2, m.pts1, m.pts2, m.offsets, ess.mask)
+
 A further view registered against the triangulated points (P3P RANSAC on 2D-3D correspondences, cv2.solvePnPRansac):
 
     view = find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=valid, px_th=2.0)
@@ -89,6 +95,7 @@ RefinedPose = collections.namedtuple("RefinedPose", "R t F cost0 cost n_used ite
 RefinedHomography = collections.namedtuple("RefinedHomography", "H cost0 cost n_used iters inliers")
 RefinedFundamental = collections.namedtuple("RefinedFundamental", "F cost0 cost n_used iters inliers")
 AbsolutePose = collections.namedtuple("AbsolutePose", "R t mask n_inliers iters cost0 cost")
+EssentialMatrix = collections.namedtuple("EssentialMatrix", "E F mask n_inliers iters cost0 cost")
 Tracks = collections.namedtuple("Tracks", "X mask n_inliers iters cost0 cost angle")
 BundleAdjustment = collections.namedtuple("BundleAdjustment", "R t X mask cost0 cost iters n_used")
 BundleAdjustmentPCG = collections.namedtuple("BundleAdjustmentPCG", "R t X mask cost0 cost iters n_used cg_iters")
@@ -657,6 +664,67 @@ def find_absolute_pose_ragged(pts2d, pts3d, K, offsets, mask=None, px_th=2.0, co
     _call(L.dgb200_find_absolute_pose_ragged_dev, L.dgb200_absolute_pose_last_error, dev, x, X, Kc, int(Kc.dim() == 3),
           off, P, rows, m, px_th, conf, max_iters, refine_iters, ds, R, t, mo, n_inl, iters, cost0, cost)
     return AbsolutePose(R, t, mo.view(torch.bool), n_inl, iters, cost0, cost)
+
+
+def find_essential_ragged(pts1, pts2, K1, K2, offsets, mask=None, px_th=1.0, conf=0.999, max_iters=10000, seeds=None,
+                          refine_iters=10):
+    """Verify calibrated image pairs: five-point MSAC-RANSAC with local optimisation over a ragged batch of
+    correspondences, the batched, device-resident counterpart of cv2.findEssentialMat.
+
+    All inputs are CUDA tensors on one device: pts1 / pts2 [rows, 2|6] (columns 0-1 are the pixel coordinates, as
+    match_descriptors_batch returns them), K1 / K2 [3,3] or [P,3,3], offsets int32 [P+1] (pair p owns rows
+    offsets[p] .. offsets[p+1]-1), mask [rows] bool / uint8 or None (every row): the rows that may be used.  Floating
+    inputs are used in float64.  A row is usable when it is in the mask and its four coordinates are finite; a pair
+    needs 5 usable rows.  px_th: the inlier threshold on the Sampson error in pixels (> 0), the F RANSAC's rule;
+    conf in (0, 1]; max_iters >= 1 bounds the RANSAC iterations; seeds: the seed of each pair's sample stream, as
+    findFundamentalMatrixBatch takes it; refine_iters >= 0 bounds the trial steps of each Levenberg-Marquardt round of
+    the local optimisation over (R, t) (0 skips it).  The estimator, its stopping rule and its local optimisation are
+    specified in include/degensac_b200.h.
+    Returns EssentialMatrix(E, F, mask, n_inliers, iters, cost0, cost): E [P,3,3] at unit Frobenius norm
+    (x2n^T E x1n = 0 for the normalised coordinates K^-1 [x, y, 1]); F [P,3,3] = K2^-T E K1^-1 at unit norm, what
+    pose_from_fundamental_ragged, refine_pose_ragged and match_descriptors_guided(..., guide="F") take; mask [rows] bool
+    the inliers of the returned model; n_inliers [P] int32; iters [P] int32 the RANSAC iterations drawn; cost0 [P] the
+    MSAC cost sum min(e^2, px_th^2) of the best RANSAC model and cost [P] that of the returned model after local
+    optimisation (cost <= cost0).  A pair without a model (fewer than 5 usable rows, no solution found, malformed
+    offsets) gets E = F = 0, no inliers and NaN costs.  The result of a pair does not depend on the batch it is in.
+    Asynchronous, nothing is read back."""
+    import torch
+    from .tensor_api import _seeds_tensor
+    named = (("pts1", pts1), ("pts2", pts2), ("K1", K1), ("K2", K2), ("offsets", offsets))
+    _check_tensors(named, mask)
+    P = _check_offsets(offsets, "P")
+    rows, dim = _check_points(pts1, pts2)
+    _check_K("K1", K1, "P", P)
+    _check_K("K2", K2, "P", P)
+    _check_floating(named[:4])
+    _check_mask(mask, "rows", rows)
+    px_th = _check_px_th(px_th, True)
+    conf = _check_conf(conf)
+    max_iters = _check_count("max_iters", max_iters, 1)
+    refine_iters = _check_count("refine_iters", refine_iters, 0)
+    dev = _check_device(named, mask)
+    if isinstance(seeds, torch.Tensor) and seeds.is_cuda and seeds.device != dev:
+        raise ValueError("seeds must be on the device of pts1")
+    per_pair = K1.dim() == 3 or K2.dim() == 3
+    if per_pair:
+        K1, K2 = K1.expand(P, 3, 3), K2.expand(P, 3, 3)
+    x1, x2, K1c, K2c = _f64(pts1[:, :2], pts2[:, :2], K1, K2)
+    off, m = offsets.contiguous(), _mask_u8(mask)
+    ds = _seeds_tensor(seeds, P, dev)
+    if tuple(ds.shape) != (P,):
+        raise ValueError("seeds must hold one seed per pair (%d), not %s" % (P, list(ds.shape)))
+    f64 = torch.float64
+    L = _cabi.lib()
+    E = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    F = torch.empty((P, 3, 3), dtype=f64, device=dev)
+    mo = _rows_out(rows, dev)
+    n_inl = torch.empty(P, dtype=torch.int32, device=dev)
+    iters = torch.empty(P, dtype=torch.int32, device=dev)
+    cost0 = torch.empty(P, dtype=f64, device=dev)
+    cost = torch.empty(P, dtype=f64, device=dev)
+    _call(L.dgb200_find_essential_ragged_dev, L.dgb200_essential_last_error, dev, x1, x2, K1c, K2c, int(per_pair), off,
+          P, rows, m, px_th, conf, max_iters, refine_iters, ds, E, F, mo, n_inl, iters, cost0, cost)
+    return EssentialMatrix(E, F, mo.view(torch.bool), n_inl, iters, cost0, cost)
 
 
 def _check_tracks(cams, pts, R, t, K, offsets):
